@@ -46,6 +46,7 @@ struct DevCfg {  // small POD, lives in global memory, hot parts copied to smem
   int32_t park_mates;                       // measurement knob (ARMADA_PARK_MATES): see Batch::produce
   int32_t collect_excl;                     // keep NumExcludedNodesByReason of the jobs that fail (DevPtrs.excl)
   int32_t k32_ok;                           // … and the resource fields without guard bits fit 26 bits (32-bit compare keys)
+  int32_t lookahead;                        // the SWAR fast loop decides the second placement of each pair ahead (off: ARMADA_NO_LOOKAHEAD)
   int32_t priorities[ARMADA_MAX_PRIORITIES];
   ArmadaPriorityClass pcs[ARMADA_MAX_PRIORITY_CLASSES];
   int64_t total_resources[ARMADA_MAX_RESOURCES];

@@ -43,10 +43,8 @@ struct DevCfg {  // small POD, lives in global memory, hot parts copied to smem
   int32_t exact;                            // exact mode (see armada_host.inc "domain"): raw units everywhere, probes are literal
                                             // ordered walks over per-level rounded keys (Ctl::scan_probe_exact), no sorted index / batches
   int64_t index_res[ARMADA_MAX_RESOURCES];  // exact mode: index resolution of the i-th indexed resource (raw units)
-  int32_t park_mates;                       // measurement knob (ARMADA_PARK_MATES): see Batch::produce
   int32_t collect_excl;                     // keep NumExcludedNodesByReason of the jobs that fail (DevPtrs.excl)
   int32_t k32_ok;                           // … and the resource fields without guard bits fit 26 bits (32-bit compare keys)
-  int32_t lookahead;                        // the SWAR fast loop decides the second placement of each pair ahead (off: ARMADA_NO_LOOKAHEAD)
   int32_t priorities[ARMADA_MAX_PRIORITIES];
   ArmadaPriorityClass pcs[ARMADA_MAX_PRIORITY_CLASSES];
   int64_t total_resources[ARMADA_MAX_RESOURCES];

@@ -317,8 +317,10 @@ typedef struct {
                                     batches, 7 pipeline epilogue.  phase_cycles[4] = iterations run in
                                     batch mode */
   uint64_t batch_debug[8];       /* device only: 0 assignment loop busy cycles, 1 assignment loop cycles
-                                    waiting for records, 2 pipeline runs, 3 batches cut short, 6 candidate
-                                    refills from the sorted index, 7 cycles spent in them; 4, 5 spare */
+                                    waiting for records, 2 pipeline runs, 3 batches cut short, 4 slow
+                                    steps of the assignment loop (supply groups given new candidates),
+                                    5 cycles spent in them, 6 candidate refills from the sorted index,
+                                    7 cycles spent in them (4-7: the SWAR form of the loop only) */
 } ArmadaRoundStats;
 
 /* ---- product entry points (libarmada_b200.so) ------------------------------------- */

@@ -130,7 +130,7 @@ def test_runs_of_known_unschedulable_jobs(n_nodes):
 def test_partly_indexed_resources(seed, indexed, lane_order):
     """Not every resource is part of the best-fit key (nodedb indexedResources ⊂ resources): the
     key no longer carries the whole row, so the SWAR shortcuts are off and the assignment table
-    keeps rows beside the keys (table_assign<false>, row-reading cursor refills)."""
+    keeps rows beside the keys (Batch::chain_run, row-reading cursor refills)."""
     batchy = seed != 403
     r = synth.random_round(seed, n_nodes=120, n_queues=6, n_jobs=900, n_running=0 if batchy else 200, gangs=not batchy, priorities=not batchy)
     r.indexed = indexed

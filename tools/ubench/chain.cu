@@ -1,12 +1,12 @@
 // Miniatures of the node-assignment chain (DESIGN.md §5.3) on ONE warp: cycles per placement for
-//   A  64-bit guard key, two redux.sync           (chain_swar<K64>, place() loop)
-//   B  32-bit compact compare key, one redux.sync (chain_swar<K32>, place() loop)
+//   A  64-bit guard key, two redux.sync, one placement after the other (the previous place() loop, K64)
+//   B  32-bit compact compare key, one redux.sync, one placement after the other (the previous place() loop, K32)
 //   C  B with the second placement of each pair decided ahead: both of its compare values (the lane
 //      won the first one / it did not) are ready before the first minimum arrives (chain_swar<K32>, place_pair)
 //   D  B with every placement decided one record ahead, one placement per loop trip
 // with the rare paths out of line behind unlikely branches, records prefetched two ahead.  The rare
 // path takes and returns the loop state by value: passing its address would keep the state in local
-// memory and put a memory round trip on the chain.
+// memory and put a memory round trip on the chain.  C, the fastest of B, C and D, is the kernel's form.
 //   nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o tools/ubench/chain tools/ubench/chain.cu && tools/ubench/chain
 #include <cstdio>
 #include <cuda_runtime.h>

@@ -48,7 +48,7 @@ __global__ void k_lat(long long* out, unsigned seed) {
 
   t0 = clock64();
 #pragma unroll 8
-  for (int i = 0; i < N; ++i) y = warp_min_u64(y + l) + 1ull;  // the 64-bit arg-min of table_assign
+  for (int i = 0; i < N; ++i) y = warp_min_u64(y + l) + 1ull;  // the 64-bit arg-min of the assignment loop (K64, chain_run)
   t1 = clock64();
   if (l == 0) out[3] = t1 - t0;
 

@@ -88,6 +88,7 @@ class RawRound:
     global_inf: bool = True
     indexed: Optional[Sequence[int]] = None             # indexed resources (default: all of them)
     resolution: Optional[Sequence[int]] = None          # index resolution per entry of `indexed` (default: TestResources)
+    drf_multipliers: Optional[Sequence[float]] = None   # [D] (default: every resource counts with weight 1)
     name: str = ""
     _keep: list = field(default_factory=list)
 
@@ -104,6 +105,7 @@ class RawRound:
 
         inp = abi.RoundInput()
         inp.abi_version = abi.ABI_VERSION
+        D = self.node_total.shape[0]
         inp.num_resources = D
         indexed = list(self.indexed) if self.indexed is not None else INDEXED
         inp.num_indexed = len(indexed)
@@ -131,7 +133,7 @@ class RawRound:
         total = self.node_allocatable.sum(axis=1)
         for d in range(D):
             inp.total_resources[d] = int(total[d])
-            inp.drf_multipliers[d] = 1.0
+            inp.drf_multipliers[d] = float(self.drf_multipliers[d]) if self.drf_multipliers is not None else 1.0
             inp.max_resources_to_schedule[d] = int(self.round_limit[d]) if self.round_limit is not None else I64_MAX
         inp.has_round_limit = 1
         inp.prefer_large_job_ordering = int(self.prefer_large)

@@ -13,7 +13,9 @@ import pytest
 import emu_lib
 import go_tables as gt
 import oracle_lib
+import shape_cases
 from armada_b200 import abi, synth
+from shape_cases import compare_key  # noqa: F401  (fixture)
 
 _dev = None
 
@@ -139,64 +141,14 @@ def test_partly_indexed_resources(seed, indexed, lane_order):
         assert int(got.stats.phase_cycles[4]) > 0
 
 
-@pytest.fixture(params=["k32", "k64"])
-def compare_key(request):
-    """The assignment loop compares 32-bit compact keys when the resource fields fit 26 bits
-    (ARMADA_NO_K32 forces the general 64-bit form)."""
-    if request.param == "k64":
-        os.environ["ARMADA_NO_K32"] = "1"
-    yield request.param
-    os.environ.pop("ARMADA_NO_K32", None)
-
-
 @pytest.mark.parametrize("wq,seed", [(8, 500), (8, 501), (16, 502), (8, 503)])
 def test_long_batch_pipelines(wq, seed, lane_order, compare_key):
-    """Small batches (ARMADA_BT_WQ test knob: items per queue per batch) make one pipeline run span
-    many batches: batch k+1 is produced from the speculative queue state while batch k is assigned,
-    jobs that find no node cut a batch short (the batch built behind it is dropped), runs of
-    known-unschedulable jobs sit between committed items."""
-    os.environ["ARMADA_BT_WQ"] = str(wq)
-    try:
-        dev = emu_lib.emu_round()
-        if seed == 503:
-            r = synth.unfeasible_runs_round(7)
-        else:
-            r = synth.random_round(seed, n_nodes=24 + 10 * (seed % 3), n_queues=5 + seed % 4, n_jobs=1400, n_running=0, gangs=seed == 502,
-                                   priorities=False, round_limit=seed == 501)
-        inp = r.to_input()
-        want = oracle_lib.round_schedule(inp)
-        got = dev.schedule(inp)
-        bad = got.diff(want)
-        assert not bad, f"{r.name}: emulated kernel != oracle:\n  " + "\n  ".join(bad)
-        if seed != 503:
-            assert int(got.stats.batch_cycles[6]) >= {500: 8, 501: 2, 502: 3}[seed], "expected several batches per pipeline run"
-        dev.close()
-    finally:
-        os.environ.pop("ARMADA_BT_WQ", None)
+    shape_cases.long_batch_pipeline(emu_lib.emu_round, wq, seed)
 
 
 @pytest.mark.parametrize("nodes,queues,jobs,wq,seed", [(60, 4, 1500, 0, 1), (120, 8, 3000, 8, 2), (250, 6, 5000, 16, 3), (40, 3, 900, 0, 4)])
 def test_gangs_as_batch_items(nodes, queues, jobs, wq, seed, lane_order, compare_key):
-    """Simple gangs (complete, one class, contiguous in their queue — what the C4 generator makes) are
-    ordered by the batch pipeline as ONE item and placed member by member by the assignment loop, all or
-    nothing: the clusters here fill up, so gangs fail in the middle (roll-back of the table, of the
-    touched bits and of the window a refill replaced) and the general loop fails them the reference's way."""
-    if wq:
-        os.environ["ARMADA_BT_WQ"] = str(wq)
-    try:
-        dev = emu_lib.emu_round()
-        r = synth.config_c4(nodes, queues, jobs, seed=synth.SEED + seed)
-        inp = r.to_input()
-        want = oracle_lib.round_schedule(inp)
-        got = dev.schedule(inp)
-        bad = got.diff(want)
-        assert not bad, f"C4 {nodes}x{jobs}: emulated kernel != oracle:\n  " + "\n  ".join(bad)
-        # gang members were placed in batch mode: more placements than iterations there
-        assert int(got.stats.placements) > int(got.stats.loop_iterations) - int(np.count_nonzero(np.asarray(want.job_state) == 4))
-        assert int(got.stats.phase_cycles[4]) > 0
-        dev.close()
-    finally:
-        os.environ.pop("ARMADA_BT_WQ", None)
+    shape_cases.gangs_as_batch_items(emu_lib.emu_round, nodes, queues, jobs, wq, seed)
 
 
 @pytest.mark.parametrize("seed", range(10))
@@ -221,16 +173,7 @@ def test_exact_mode_resolution_rounding_blocks_a_feasible_node():
 
 @pytest.mark.parametrize("seed", [0, 5])
 def test_exact_mode_forced_on_aligned_rounds(seed):
-    """ARMADA_FORCE_EXACT: the literal walk on inputs the fast path also accepts gives the same round."""
-    os.environ["ARMADA_FORCE_EXACT"] = "1"
-    try:
-        dev = emu_lib.emu_round()
-        r = synth.random_round(seed, away=(seed % 4 == 1), n_nodes=60, n_jobs=350, n_running=90, protected_fraction=0.5 if seed else 0.0)
-        inp = r.to_input()
-        assert not dev.schedule(inp).diff(oracle_lib.round_schedule(inp))
-        dev.close()
-    finally:
-        os.environ.pop("ARMADA_FORCE_EXACT", None)
+    shape_cases.exact_mode_forced(emu_lib.emu_round, seed)
 
 
 def test_more_classes_than_the_shared_memory_table_holds():
@@ -521,3 +464,52 @@ def test_dry_run_nodedb_ignores_floating_resources_in_the_node_fit():
     gangs = [[j] for j in with_lic[:10]] + [[j] for j in range(J) if b.jobs[j].node is None][:10]
     oks = _dry_run_case(_R(b), gangs, emu_lib.load())
     assert all(oks[: len(with_lic[:10])])  # 1–16 cpu on 32-cpu nodes of an empty cluster: every one fits
+
+
+# ---- every resource count and key layout (tests/shape_cases.py) ------------------------------------------
+def _shape_params():
+    """Every case once; the batch cases at D = 1 and D = 8 also with the lanes of every warp in reverse order."""
+    out = []
+    for c in shape_cases.MATRIX:
+        orders = ("forward", "reverse") if c.kind == "batch" and c.D in (1, 8) else ("forward",)
+        out += [pytest.param(c, o, id=f"{c.id}-{o}") for o in orders]
+    return out
+
+
+@pytest.mark.parametrize("case,order", _shape_params())
+def test_resource_counts_and_key_layouts(case, order, capfd, monkeypatch):
+    """k_schedule_pass<1|2|4|8> with each assignment-loop form (K32, K64, chain_run with unindexed resources or
+    without guard bits, exact mode), field widths at the K32 / K64 boundaries, classes of exactly the largest
+    node and larger than every node, index orders that differ from the resource order, 1–33 and 4097 nodes, DRF
+    multipliers 0 / 0.5 / 3 with a licence as the dominant resource: the layout the case was built for, and
+    every output array equal to the oracle's."""
+    monkeypatch.setenv("EMU_ORDER", order)
+    shape_cases.check_case(case, emu_lib.emu_round(), oracle_lib.round_schedule, capfd)
+
+
+@pytest.mark.parametrize("case", [shape_cases.REFUSED, shape_cases.REFUSED_COARSENED, shape_cases.REFUSED_UNINDEXED], ids=lambda c: c.id)
+def test_key_wider_than_63_bits_is_refused(case, capfd):
+    """A best-fit key wider than 63 bits is refused with E_UNSUPPORTED and nothing is computed; the same nodes and
+    jobs with the widest field coarsened, or not indexed, are scheduled bit-exactly."""
+    shape_cases.check_case(case, emu_lib.emu_round(), oracle_lib.round_schedule, capfd)
+
+
+def test_shape_matrix_is_covered(capfd):
+    """The case generator reaches every (instantiation, assignment-loop form) pair it is meant to, and the refusal:
+    an edit that quietly drops a path fails here."""
+    dev = emu_lib.emu_round()
+    reached = set()
+    for c in shape_cases.MATRIX:
+        inp = shape_cases.shape_round(c).to_input()
+        capfd.readouterr()
+        with shape_cases.knob("ARMADA_TIME_UPLOAD", 1):
+            dev.upload(inp)
+        form = shape_cases.form_of(shape_cases.layout_of(capfd.readouterr().err), inp)
+        assert form == c.form, c.id
+        reached.add((shape_cases.instantiation(c.D), form))
+    assert reached == shape_cases.expected_pairs(), sorted(reached ^ shape_cases.expected_pairs())
+    with pytest.raises(abi.ArmadaError) as ei:
+        dev.upload(shape_cases.shape_round(shape_cases.REFUSED).to_input())
+    assert ei.value.status == abi.E_UNSUPPORTED
+    dev.close()
+    print("reached:", ", ".join(f"<{i}> {f}" for i, f in sorted(reached)), "+ the 63-bit refusal")

@@ -7,8 +7,10 @@ import pytest
 
 import go_tables as gt
 import oracle_lib
+import shape_cases
 from armada_b200 import abi, synth
 from armada_b200.scheduler import DeviceRound
+from shape_cases import Case, compare_key  # noqa: F401  (fixture)
 
 pytestmark = pytest.mark.gpu
 
@@ -392,3 +394,71 @@ def test_job_priority_comparer_on_device(name):
     b, expected = order_cases.comparison_round(name)
     got, _ = assert_parity(b.input, name)
     order_cases.check_order(b, expected, got)
+
+
+# ---- every resource count and key layout (tests/shape_cases.py), and the emulator's knob tests on the device ----
+GPU_SHAPES = shape_cases.MATRIX + [
+    # queue counts: the window width and the batch width switch with them (1 queue, more than 64, the maximum)
+    Case(1, "k32", "batch", 200, n_nodes=300, n_queues=1, n_jobs=2500),
+    Case(8, "k32", "batch", 201, n_nodes=300, n_queues=65, n_jobs=2500),
+    Case(4, "k64", "batch", 202, n_nodes=300, n_queues=100, n_jobs=2500),
+    Case(5, "k32", "batch", 203, n_nodes=300, n_queues=128, n_jobs=2500),
+    Case(8, "run", "eviction", 204, n_nodes=300, n_queues=128, n_jobs=2500),
+    # thousands of nodes: more than one tile group, hundreds of batches
+    Case(8, "k32", "batch", 210, n_nodes=4097, n_queues=9, n_jobs=20000),
+    Case(1, "k32", "batch", 211, n_nodes=4097, n_queues=9, n_jobs=20000),
+    Case(8, "k64", "batch", 212, n_nodes=4500, n_queues=9, n_jobs=20000),
+    Case(1, "k64", "batch", 213, n_nodes=3000, n_queues=9, n_jobs=20000),
+    Case(8, "k32", "eviction", 214, n_nodes=3000, n_queues=9, n_jobs=6000),
+    Case(1, "k32", "eviction", 215, n_nodes=5000, n_queues=9, n_jobs=6000),
+]
+
+
+@pytest.mark.parametrize("case", GPU_SHAPES, ids=lambda c: c.id)
+def test_resource_counts_and_key_layouts(case, capfd):
+    """k_schedule_pass<1|2|4|8> with each assignment-loop form (K32, K64, chain_run with unindexed resources or
+    without guard bits, exact mode), field widths at the K32 / K64 boundaries, 1 to 5000 nodes, 1 to 128 queues,
+    DRF multipliers 0 / 0.5 / 3 with a licence as the dominant resource: the layout the case was built for, and
+    every output array equal to the oracle's."""
+    shape_cases.check_case(case, device(), oracle_lib.round_schedule, capfd)
+
+
+@pytest.mark.parametrize("case", [shape_cases.REFUSED, shape_cases.REFUSED_COARSENED, shape_cases.REFUSED_UNINDEXED], ids=lambda c: c.id)
+def test_key_wider_than_63_bits_is_refused(case, capfd):
+    with DeviceRound(0) as dev:
+        shape_cases.check_case(case, dev, oracle_lib.round_schedule, capfd)
+
+
+@pytest.mark.parametrize("case", [Case(8, "k32", "batch", 220, n_nodes=600, n_jobs=8000), Case(1, "k32", "batch", 221, n_nodes=600, n_jobs=8000)],
+                         ids=lambda c: c.id)
+def test_shape_rounds_are_deterministic(case):
+    """A D = 8 and a D = 1 batch round repeated on one handle: bit-identical every time, and equal to the oracle."""
+    inp = shape_cases.shape_round(case).to_input()
+    with DeviceRound(0) as dev:
+        dev.upload(inp)
+        ref = None
+        for _ in range(4):
+            st = dev.run()
+            got = dev.download()
+            if ref is None:
+                ref = got
+            else:
+                assert not got.diff(ref)
+    assert int(st.phase_cycles[4]) > 0
+    assert not ref.diff(oracle_lib.round_schedule(inp))
+
+
+@pytest.mark.parametrize("wq,seed", [(8, 500), (8, 501), (16, 502), (8, 503)])
+def test_long_batch_pipelines(wq, seed, compare_key):
+    shape_cases.long_batch_pipeline(lambda: DeviceRound(0), wq, seed)
+
+
+@pytest.mark.parametrize("nodes,queues,jobs,wq,seed", [(60, 4, 1500, 0, 1), (120, 8, 3000, 8, 2), (250, 6, 5000, 16, 3), (40, 3, 900, 0, 4)])
+def test_gangs_as_batch_items_with_knobs(nodes, queues, jobs, wq, seed, compare_key):
+    """test_gangs_as_batch_items with small batches (ARMADA_BT_WQ) and the 64-bit compare keys (ARMADA_NO_K32)."""
+    shape_cases.gangs_as_batch_items(lambda: DeviceRound(0), nodes, queues, jobs, wq, seed)
+
+
+@pytest.mark.parametrize("seed", [0, 5])
+def test_exact_mode_forced_on_aligned_rounds(seed):
+    shape_cases.exact_mode_forced(lambda: DeviceRound(0), seed)

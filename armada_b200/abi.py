@@ -11,6 +11,7 @@ ABI_VERSION = 2
 MAX_RESOURCES = 8
 EXCLUDED_KINDS = 5  # ARMADA_EXCL_*: node type, static, resources (reached), implicit, disallowed
 EXCL_NODE_TYPE, EXCL_STATIC, EXCL_RESOURCES, EXCL_IMPLICIT, EXCL_DISALLOWED = range(5)
+EXCL_STATIC_TOTAL = 5  # ExcludedReason.kind only: counted as EXCL_RESOURCES in the round's histogram
 MAX_PRIORITIES = 16
 MAX_PRIORITY_CLASSES = 32
 MAX_AWAY = 4
@@ -183,6 +184,16 @@ class RoundStats(C.Structure):
     ]
 
 
+class ExcludedReason(C.Structure):
+    _fields_ = [
+        ("kind", C.c_uint32),
+        ("sub", C.c_uint32),
+        ("quantity", C.c_int64),
+        ("count", C.c_uint32),
+        ("_pad", C.c_uint32),
+    ]
+
+
 REPO_ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 PRODUCT_LIB_PATH = os.path.join(REPO_ROOT, "armada_b200", "libarmada_b200.so")
 
@@ -216,6 +227,8 @@ def declare_prototypes(lib: C.CDLL) -> None:
     lib.armada_nodedb_create.restype = C.c_int32
     lib.armada_nodedb_schedule_many.argtypes = [vp, C.c_uint32, u32p, u32p, u8p, u32p]
     lib.armada_nodedb_schedule_many.restype = C.c_int32
+    lib.armada_nodedb_explain.argtypes = [vp, C.c_uint32, u32p, u32p, u8p, u32p, u32p, u8p, u32p, C.POINTER(ExcludedReason), C.c_uint32, u32p]
+    lib.armada_nodedb_explain.restype = C.c_int32
     lib.armada_nodedb_select_nodes.argtypes = [vp, C.c_uint32, u32p, u32p]
     lib.armada_nodedb_select_nodes.restype = C.c_int32
     lib.armada_nodedb_destroy.argtypes = [vp]
@@ -253,6 +266,7 @@ PRODUCT_SYMBOLS = [
     "armada_round_schedule",
     "armada_nodedb_create",
     "armada_nodedb_schedule_many",
+    "armada_nodedb_explain",
     "armada_nodedb_select_nodes",
     "armada_nodedb_destroy",
     "armada_strerror",

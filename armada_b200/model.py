@@ -970,3 +970,144 @@ def queue_stats(b: "RoundInputBuilder", res: "RoundResult") -> Dict[str, QueueSt
                 st.last_gang_scheduled_queue_cost = cost / float(b.qw[qi])
         out[q.name] = st
     return out
+
+
+# ---- the reference's exclusion reason strings (nodedb/nodematching.go:14-122, context/pod.go:58-80) ----------
+_DEC_SUFFIX = {-9: "n", -6: "u", -3: "m", 0: "", 3: "k", 6: "M", 9: "G", 12: "T", 15: "P", 18: "E"}
+
+
+def quantity_string(value: int, scale: int) -> str:
+    """`resource.NewScaledQuantity(value, scale).String()` — how `ResourceList.asQuantity` prints
+    (internaltypes/resource_list.go:292-297).  Restated from apimachinery's Quantity.CanonicalizeBytes and
+    int64Amount.AsCanonicalBytes (read, not executed): a DecimalSI quantity strips trailing zeros of the
+    value into the exponent, then multiplies back until the exponent is a multiple of 3, and prints the
+    integer with the SI suffix of that exponent; zero is "0".  Exponents outside n…E never arise from an
+    int64 at the factory's scales and are refused."""
+    value, exp = int(value), int(scale)
+    if value == 0:
+        return "0"
+    while value % 10 == 0:
+        value //= 10
+        exp += 1
+    r = exp % 3  # Python's modulo is non-negative: 1 ↔ Go's {1, -2}, 2 ↔ {2, -1}
+    value *= 10 ** r
+    exp -= r
+    if exp not in _DEC_SUFFIX:
+        raise ValueError(f"quantity {value}e{exp} has no DecimalSI suffix")
+    return f"{value}{_DEC_SUFFIX[exp]}"
+
+
+def untolerated_taint_reason(t: Taint) -> str:  # UntoleratedTaint.String
+    return f"taint {t.key}={t.value}:{t.effect} not tolerated"
+
+
+def missing_label_reason(label: str) -> str:  # MissingLabel.String
+    return f"node does not match pod NodeSelector: label {label} not set"
+
+
+def unmatched_label_reason(label: str, pod_value: str, node_value: str) -> str:  # UnmatchedLabel.String
+    return f"node does not match pod NodeSelector: required label {label} = {pod_value}, but node has {node_value}"
+
+
+def node_selector_string(terms: Sequence[Tuple[MatchExpression, ...]]) -> str:
+    """`(*v1.NodeSelector).String()` as printed by UnmatchedNodeSelector (`%s`): the gogo-protobuf
+    generated String of k8s.io/api/core/v1 (generated.pb.go; restated from reading it)."""
+    def req(e: MatchExpression) -> str:
+        return f"NodeSelectorRequirement{{Key:{e.key},Operator:{e.operator},Values:[{' '.join(e.values)}],}}"
+    out = "&NodeSelector{NodeSelectorTerms:[]NodeSelectorTerm{"
+    for term in terms:
+        out += "NodeSelectorTerm{MatchExpressions:[]NodeSelectorRequirement{" + "".join(req(e) + "," for e in term) + "},"
+        out += "MatchFields:[]NodeSelectorRequirement{},},"
+    return out + "},}"
+
+
+def insufficient_resources_reason(name: str, required: str, available: str) -> str:  # InsufficientResources.String
+    return f"pod requires {required} {name}, but only {available} is available"
+
+
+def _selector_reason(selector: Sequence[Tuple[str, str]], labels: Dict[str, str], unset: Optional[set]) -> Optional[str]:
+    """NodeSelectorRequirementsMet (nodematching.go:215-240).  The reference ranges over the selector MAP, so
+    when several labels fail it reports one at random; this restatement takes them in label order."""
+    for label, pod_value in selector:
+        if label in labels:
+            if labels[label] != pod_value:
+                return unmatched_label_reason(label, pod_value, labels[label])
+        elif unset is None or label in unset:
+            return missing_label_reason(label)
+    return None
+
+
+def excluded_reason_string(b: "RoundInputBuilder", row: int, cls: int, rec) -> str:
+    """The reason string of one ExcludedReason record of a job of class `cls` probed with static row `row`."""
+    kind = int(rec.kind)
+    if kind == abi.EXCL_IMPLICIT:
+        return "insufficient resources available"  # PodRequirementsNotMetReasonInsufficientResources
+    if kind == abi.EXCL_DISALLOWED:
+        return "job requests disallowed resource and therefore cannot be scheduled"  # disallowedResourceRequested, nodedb.go:26
+    tolerations, selector, affinity = b.row_specs[row]
+    if kind == abi.EXCL_NODE_TYPE:  # NodeTypeJobRequirementsMet (:127-139)
+        taints, labels, unset = b.type_specs[int(rec.sub)]
+        t = find_untolerated(taints, tolerations)
+        if t is not None:
+            return untolerated_taint_reason(t)
+        r = _selector_reason(selector, labels, unset)
+        if r is None:
+            raise ValueError(f"node type {int(rec.sub)} matches row {row}")
+        return r
+    if kind == abi.EXCL_STATIC:  # StaticJobRequirementsMet's string predicates (:161-181)
+        taints, labels = b.static_specs[int(rec.sub)]
+        t = find_untolerated(taints, tolerations)
+        if t is not None:
+            return untolerated_taint_reason(t)
+        r = _selector_reason(selector, labels, None)
+        if r is not None:
+            return r
+        if affinity is not None and not match_node_selector_terms(labels, affinity):
+            return "node does not match pod NodeAffinity " + node_selector_string(affinity)
+        raise ValueError(f"static class {int(rec.sub)} matches row {row}")
+    # ARMADA_EXCL_STATIC_TOTAL / ARMADA_EXCL_RESOURCES: InsufficientResources (resource_list.go:167-191)
+    d = int(rec.sub)
+    f = b.factory
+    return insufficient_resources_reason(f.names[d], quantity_string(int(b.class_request[cls, d]), f.scales[d]),
+                                         quantity_string(int(rec.quantity), f.scales[d]))
+
+
+def pod_scheduling_context_string(num_nodes: int, excluded: Dict[str, int], node_id: str = "") -> str:
+    """PodSchedulingContext.String (context/pod.go:62-81) through text/tabwriter(minwidth 1, tabwidth 1,
+    padding 1, ' ', 0): each column of a run of lines that have a cell there is as wide as its widest
+    cell plus one.  The reference ranges over the excluded-nodes MAP, so its lines come in random order;
+    here they come in reason-string order."""
+    head = [("Node:", node_id or "none"), ("Number of nodes in cluster:", str(num_nodes))]
+    if not excluded:
+        head.append(("Excluded nodes:", "none"))  # a cell of the first column too
+    w0 = max(len(a) for a, _ in head) + 1
+    out = "".join(a.ljust(w0) + v + "\n" for a, v in head)
+    if not excluded:
+        return out
+    out += "Excluded nodes:\n"
+    items = sorted(excluded.items())
+    w1 = max(len(f"{c}:") for _, c in items) + 1
+    return out + "".join(" " + f"{c}:".ljust(w1) + reason + "\n" for reason, c in items)
+
+
+def last_probe_row(b: "RoundInputBuilder", cls: int) -> Optional[int]:
+    """The static row of the last probe SelectNodeForJobWithTxn runs for a single job of class `cls` that
+    fits nowhere (nodedb.go:431-512): the last away node type that adds taints when away scheduling is
+    on, else the home row when home scheduling is on; None when no probe runs."""
+    if not b.cfg.disable_away_scheduling:
+        for k in reversed(range(abi.MAX_AWAY)):
+            if int(b.class_away[cls, k]) != abi.NONE:
+                return int(b.class_away[cls, k])
+    return None if b.cfg.disable_home_scheduling else int(b.class_row[cls])
+
+
+def excluded_nodes_by_reason(b: "RoundInputBuilder", cls: int, records) -> Dict[str, int]:
+    """NumExcludedNodesByReason of a failed single job of class `cls` from its explain records: records
+    whose strings coincide (two node types with the same untolerated taint, a total and an allocatable of
+    the same quantity, …) add up, as they do under the reference's string keys."""
+    row = last_probe_row(b, cls)
+    out: Dict[str, int] = {}
+    for r in records:
+        s = excluded_reason_string(b, row, cls, r)
+        out[s] = out.get(s, 0) + int(r.count)
+    return out

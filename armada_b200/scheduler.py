@@ -12,7 +12,7 @@ import ctypes as C
 from typing import Optional
 
 from . import abi
-from .model import RoundResult
+from .model import RoundResult, excluded_nodes_by_reason
 
 
 class DeviceRound:
@@ -120,6 +120,43 @@ class DeviceNodeDb:
             raise abi.ArmadaError(st, f"{self.lib.armada_strerror(st).decode()}: {self.lib.armada_last_error().decode()}")
         out_nodes = [node[int(start[g]):int(start[g + 1])].copy() for g in range(len(gangs))]
         return ok[: len(gangs)].astype(bool), out_nodes
+
+    def explain(self, gangs, capacity: int = 1024, builder=None):
+        """`schedule_many` that also says why, in one launch (armada_nodedb_explain).  Per gang:
+        `(ok, member_node, num_placed, away, records)` — `records` is a list of abi.ExcludedReason, the
+        NumExcludedNodesByReason of a failed gang of one, empty otherwise; with the db's `builder`
+        (RoundInputBuilder) it is that map itself, {reason string: count}.  The record buffer starts at
+        `capacity` and is grown once, to the size the library reports, when it was too small."""
+        import numpy as np
+        G = len(gangs)
+        start = np.zeros(G + 1, np.uint32)
+        start[1:] = np.cumsum([len(g) for g in gangs])
+        members = np.asarray([c for g in gangs for c in g] or [0], dtype=np.uint32)
+        ok = np.zeros(max(G, 1), np.uint8)
+        node = np.full(max(int(start[-1]), 1), abi.NONE, np.uint32)
+        placed = np.zeros(max(G, 1), np.uint32)
+        away = np.zeros(max(G, 1), np.uint8)
+        rstart = np.zeros(G + 1, np.uint32)
+        needed = C.c_uint32(0)
+        cap = max(int(capacity), 1)
+        for _ in range(2):
+            recs = (abi.ExcludedReason * cap)()
+            st = self.lib.armada_nodedb_explain(self.h, G, start.ctypes.data_as(abi.u32p), members.ctypes.data_as(abi.u32p), ok.ctypes.data_as(abi.u8p),
+                                                node.ctypes.data_as(abi.u32p), placed.ctypes.data_as(abi.u32p), away.ctypes.data_as(abi.u8p),
+                                                rstart.ctypes.data_as(abi.u32p), recs, cap, C.byref(needed))
+            if st != abi.OK:
+                raise abi.ArmadaError(st, f"{self.lib.armada_strerror(st).decode()}: {self.lib.armada_last_error().decode()}")
+            if needed.value <= cap:
+                break
+            cap = needed.value
+        out = []
+        for g in range(G):
+            lo, hi = int(start[g]), int(start[g + 1])
+            rec = list(recs[int(rstart[g]):int(rstart[g + 1])])
+            if builder is not None:
+                rec = excluded_nodes_by_reason(builder, int(gangs[g][0]), rec) if rec else {}
+            out.append((bool(ok[g]), node[lo:hi].copy(), int(placed[g]), bool(away[g]), rec))
+        return out
 
     def select_nodes(self, classes):
         """One independent job per entry (its job class): the node it would be bound to on the empty

@@ -109,6 +109,28 @@ enum {
 /* kinds of ArmadaRoundOutput.job_excluded_nodes */
 #define ARMADA_EXCLUDED_KINDS 5u
 enum { ARMADA_EXCL_NODE_TYPE = 0, ARMADA_EXCL_STATIC = 1, ARMADA_EXCL_RESOURCES = 2, ARMADA_EXCL_IMPLICIT = 3, ARMADA_EXCL_DISALLOWED = 4 };
+/* armada_nodedb_explain only: the total-resources step of StaticJobRequirementsMet (nodematching.go:182-186),
+ * counted under ARMADA_EXCL_RESOURCES in the round's kind histogram */
+#define ARMADA_EXCL_STATIC_TOTAL 5u
+
+/* One key of PodSchedulingContext.NumExcludedNodesByReason with its count (armada_nodedb_explain).  The
+ * reference's key is a string; (kind, sub, quantity) is what the string is made of:
+ *   ARMADA_EXCL_NODE_TYPE     sub = node type t (NodeTypeJobRequirementsMet failed on t), count = nodes of t
+ *   ARMADA_EXCL_STATIC        sub = node static class s: the first failing taint / selector / affinity
+ *                             predicate of the job's row on a node of class s
+ *   ARMADA_EXCL_STATIC_TOTAL  sub = resource d, quantity = the node's TOTAL of d (first d over it)
+ *   ARMADA_EXCL_RESOURCES     sub = resource d, quantity = the node's allocatable of d at the probed level
+ *                             (first d in factory order the request exceeds: InsufficientResources)
+ *   ARMADA_EXCL_DISALLOWED    disallowedResourceRequested (count = every node)
+ *   ARMADA_EXCL_IMPLICIT      "insufficient resources available": the nodes no other record counts
+ * Quantities are in the factory's native scale. */
+typedef struct {
+  uint32_t kind;
+  uint32_t sub;
+  int64_t quantity;
+  uint32_t count;
+  uint32_t _pad;
+} ArmadaExcludedReason;
 
 /* node flags */
 #define ARMADA_NODE_UNSCHEDULABLE 1u /* Node.unschedulable (carries the unschedulable taint) */
@@ -369,6 +391,23 @@ int32_t armada_nodedb_create(int32_t device, const ArmadaRoundInput* in, ArmadaN
  * placed on (caller's node numbering), ARMADA_NONE for the members of the others. */
 int32_t armada_nodedb_schedule_many(ArmadaNodeDb* db, uint32_t num_gangs, const uint32_t* gang_start, const uint32_t* member_class,
                                     uint8_t* ok, uint32_t* member_node);
+/* armada_nodedb_schedule_many that also says why (what SubmitChecker.getSchedulingResult reports,
+ * submitcheck.go:382-415); ok and member_node are exactly schedule_many's.  Per gang g:
+ *   num_placed[g]  members that found a node before the first one failed (numSuccessfullyScheduled);
+ *                  the gang's size when ok[g]
+ *   away[g]        (may be NULL) ok[g] and member 0 was placed on an away node type (ScheduledAway)
+ *   reasons[reason_start[g] .. reason_start[g+1])  for a failed gang of ONE member: the
+ *                  NumExcludedNodesByReason of its PodSchedulingContext — the map of the last probe the
+ *                  reference runs (home, then each away node type), with the implicit exclusions added —
+ *                  as records sorted by (kind, sub, quantity); their counts sum to the number of nodes.
+ *                  Empty for every other gang.
+ * reason_start has num_gangs + 1 entries.  *needed = reason_start[num_gangs].  Like snprintf, the records
+ * are written only when *needed <= capacity (reasons may be NULL when capacity is 0); everything else is
+ * written either way, and a call that did not fit can be repeated with a larger buffer.  Gangs of more
+ * than 256 members are ARMADA_E_UNSUPPORTED, as in schedule_many. */
+int32_t armada_nodedb_explain(ArmadaNodeDb* db, uint32_t num_gangs, const uint32_t* gang_start, const uint32_t* member_class, uint8_t* ok,
+                              uint32_t* member_node, uint32_t* num_placed, uint8_t* away, uint32_t* reason_start, ArmadaExcludedReason* reasons,
+                              uint32_t capacity, uint32_t* needed);
 /* NodeDb.SelectNodeForJobWithTxn (nodedb.go:431-512) for num_jobs independent jobs against the empty
  * cluster — what SubmitChecker does for a single job (submitcheck.go:353-371): node[i] = the node job i
  * (a job-class index of `in`) would be bound to, ARMADA_NONE = it fits nowhere. */

@@ -45,6 +45,8 @@ struct DevCfg {  // small POD, lives in global memory, hot parts copied to smem
   int64_t index_res[ARMADA_MAX_RESOURCES];  // exact mode: index resolution of the i-th indexed resource (raw units)
   int32_t collect_excl;                     // keep NumExcludedNodesByReason of the jobs that fail (DevPtrs.excl)
   int32_t k32_ok;                           // … and the resource fields fit 26 bits without guard bits, 31 with them (32-bit compare keys)
+  int32_t min_bind_prio;                    // lowest priority a job of a preemptible class can be bound at this round, evicted jobs
+                                            // aside: running jobs' scheduled-at priorities, the classes' priority classes and away priorities
   int32_t priorities[ARMADA_MAX_PRIORITIES];
   ArmadaPriorityClass pcs[ARMADA_MAX_PRIORITY_CLASSES];
   int64_t total_resources[ARMADA_MAX_RESOURCES];

@@ -119,7 +119,7 @@ __global__ void k_reset(DevCfg c, DevPtrs P) {
   for (size_t n = i; n < c.N; n += stride) P.fp_epoch[n] = 0;
   for (size_t k = i; k < (size_t)c.C; k += stride) P.unfeasible[k] = 0;
   if (i < 16) P.counters[i] = 0;
-  if (i < 48) P.stats[i] = 0;
+  if (i < 50) P.stats[i] = 0;
 }
 
 // CreateAndInsertWithJobDbJobsWithTxn (nodedb.go:43-60): bind every running job at its

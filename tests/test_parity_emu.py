@@ -2,8 +2,9 @@
 by g++ against tools/simt_emu/cuda_emu.h (deterministic SIMT emulator, test tooling only) and
 compared bit-for-bit with the CPU oracle.  The real parity tests are tests/test_parity_gpu.py
 (pytest -m gpu, through the nvcc-built product library); this module exists so that control-flow /
-data-structure bugs in the kernels are caught on a CPU-only box.  EMU_ORDER=reverse runs the
-lanes of every warp in the opposite order (catches missing __syncwarp in either direction)."""
+data-structure bugs in the kernels are caught on a CPU-only box.  The bodies both modules run are in
+tests/round_cases.py.  EMU_ORDER=reverse runs the lanes of every warp in the opposite order (catches
+missing __syncwarp in either direction)."""
 import os
 
 import numpy as np
@@ -11,10 +12,14 @@ import numpy as np
 import pytest
 
 import emu_lib
+import gang_cases
 import go_tables as gt
 import oracle_lib
+import order_cases
+import round_cases as rc
 import shape_cases
 from armada_b200 import abi, synth
+from armada_b200.scheduler import DeviceNodeDb
 from shape_cases import compare_key  # noqa: F401  (fixture)
 
 _dev = None
@@ -27,12 +32,12 @@ def emu_round(inp):
     return _dev.schedule(inp)
 
 
+def emu_nodedb(inp):
+    return DeviceNodeDb(inp, 0, lib=emu_lib.load())
+
+
 def assert_parity(inp, label=""):
-    want = oracle_lib.round_schedule(inp)
-    got = emu_round(inp)
-    bad = got.diff(want)
-    assert not bad, f"{label}: emulated kernel != oracle:\n  " + "\n  ".join(bad)
-    return got, want
+    return rc.assert_parity(emu_round, inp, label)
 
 
 @pytest.fixture(params=["forward", "reverse"])
@@ -48,25 +53,12 @@ def lane_order(request):
 
 @pytest.mark.parametrize("seed", range(24))
 def test_random_rounds(seed, lane_order):
-    r = synth.random_round(
-        seed,
-        away=(seed % 4 == 1),
-        round_limit=(seed % 6 == 3),
-        queue_limits=(seed % 6 == 4),
-        protected_fraction=0.5 if seed % 3 == 2 else 0.0,
-        lookback=40 if seed % 5 == 1 else 0,
-        n_nodes=40 + 13 * (seed % 7),
-        n_jobs=300 + 50 * (seed % 5),
-        n_running=80 + 20 * (seed % 4),
-    )
-    assert_parity(r.to_input(), r.name)
+    rc.random_rounds(emu_round, seed)
 
 
 @pytest.mark.parametrize("seed", [100, 101])
 def test_random_rounds_many_nodes(seed):
-    r = synth.random_round(seed, n_nodes=1500 + 700 * (seed % 3), n_queues=9, n_jobs=2500, n_running=1200,
-                           protected_fraction=0.5 if seed % 2 else 0.0)
-    assert_parity(r.to_input(), r.name)
+    rc.random_rounds_many_nodes(emu_round, seed, n_nodes=1500 + 700 * (seed % 3), n_jobs=2500, n_running=1200)
 
 
 @pytest.mark.parametrize("n_queues", [40, 100, 128])
@@ -80,65 +72,28 @@ def test_many_queues(n_queues):
 
 @pytest.mark.parametrize("name,scale", [("C2", 0.02), ("C3", 0.004), ("C4", 0.006), ("C5", 0.004)])
 def test_scaled_configs(name, scale):
-    r = synth.scaled(name, scale)
-    got, want = assert_parity(r.to_input(), f"{name}@{scale}")
-    assert got.out.num_result_scheduled == want.out.num_result_scheduled
+    rc.scaled_config(emu_round, name, scale)
 
 
-PQS = gt.load_cases("preempting_queue_scheduler")
-QS = gt.load_cases("queue_scheduler")
-
-
-def _emu_round_or_skip(inp):
-    try:
-        got = emu_round(inp)
-    except abi.ArmadaError as e:
-        if e.status == abi.E_UNSUPPORTED:
-            raise gt.UnsupportedCase(str(e))
-        raise
-    want = oracle_lib.round_schedule(inp)
-    bad = got.diff(want)
-    assert not bad, "emulated kernel != oracle:\n  " + "\n  ".join(bad)
-    return got
-
-
-@pytest.mark.parametrize("name", sorted(PQS.keys()))
+@pytest.mark.parametrize("name", sorted(rc.PQS.keys()))
 def test_reference_pqs_tables(name):
-    try:
-        gt.run_pqs_case(PQS[name], _emu_round_or_skip)
-    except gt.UnsupportedCase as e:
-        pytest.skip(f"outside device domain / not modelled: {e}")
+    rc.reference_table(emu_round, gt.run_pqs_case, rc.PQS[name])
 
 
-@pytest.mark.parametrize("name", sorted(QS.keys()))
+@pytest.mark.parametrize("name", sorted(rc.QS.keys()))
 def test_reference_queue_scheduler_tables(name):
-    try:
-        gt.run_queue_scheduler_case(QS[name], _emu_round_or_skip)
-    except gt.UnsupportedCase as e:
-        pytest.skip(f"outside device domain / not modelled: {e}")
+    rc.reference_table(emu_round, gt.run_queue_scheduler_case, rc.QS[name])
 
 
 @pytest.mark.parametrize("n_nodes", [7, 401])
 def test_runs_of_known_unschedulable_jobs(n_nodes):
-    """synth.unfeasible_runs_round: skipped runs around the 128-record fast-forward step; the level
-    scan that proves the miss covers node counts that are not a multiple of its stride."""
-    r = synth.unfeasible_runs_round(n_nodes)
-    got, want = assert_parity(r.to_input(), r.name)
-    assert got.out.num_result_scheduled == want.out.num_result_scheduled == 11 + 40
+    rc.runs_of_known_unschedulable_jobs(emu_round, n_nodes)
 
 
 @pytest.mark.parametrize("seed,indexed", [(400, [synth.CPU, synth.MEM]), (401, [synth.CPU]), (402, [synth.MEM, synth.GPU]),
                                           (403, [synth.CPU, synth.MEM])])
 def test_partly_indexed_resources(seed, indexed, lane_order):
-    """Not every resource is part of the best-fit key (nodedb indexedResources ⊂ resources): the
-    key no longer carries the whole row, so the SWAR shortcuts are off and the assignment table
-    keeps rows beside the keys (Batch::chain_run, row-reading cursor refills)."""
-    batchy = seed != 403
-    r = synth.random_round(seed, n_nodes=120, n_queues=6, n_jobs=900, n_running=0 if batchy else 200, gangs=not batchy, priorities=not batchy)
-    r.indexed = indexed
-    got, _ = assert_parity(r.to_input(), f"{r.name} indexed={indexed}")
-    if batchy:
-        assert int(got.stats.phase_cycles[4]) > 0
+    rc.partly_indexed_resources(emu_round, seed, indexed)
 
 
 @pytest.mark.parametrize("wq,seed", [(8, 500), (8, 501), (16, 502), (8, 503)])
@@ -153,22 +108,11 @@ def test_gangs_as_batch_items(nodes, queues, jobs, wq, seed, lane_order, compare
 
 @pytest.mark.parametrize("seed", range(10))
 def test_exact_mode_unaligned_rounds(seed, lane_order):
-    """Inputs outside the fast domain run in exact mode: the reference's default index resolutions
-    (cpu 100m, memory 100Mi) with 250m / 4Gi-style requests, node sizes that are not multiples of
-    them, allocatable < total, a NodeFactory index order that differs from the node-id order, classes
-    that match several node types.  Every probe is the literal ordered walk of nodeiteration.go."""
-    r = synth.random_round(seed, away=(seed % 4 == 1), n_nodes=40 + 13 * (seed % 7), n_jobs=300 + 50 * (seed % 5),
-                           n_running=80 + 20 * (seed % 4), protected_fraction=0.5 if seed % 3 == 2 else 0.0,
-                           round_limit=(seed % 6 == 3), queue_limits=(seed % 6 == 4), lookback=40 if seed % 5 == 1 else 0, unaligned=True)
-    assert_parity(r.to_input(), r.name)
+    rc.exact_mode_unaligned_round(emu_round, seed)
 
 
 def test_exact_mode_resolution_rounding_blocks_a_feasible_node():
-    """gang_scheduler_test.go:244-262 on the device path: the fourth job fits a node but the rounded
-    index key hides that node from the iterator."""
-    got, want = assert_parity(synth.rounding_round().to_input(), "rounding")
-    assert got.out.num_result_scheduled == want.out.num_result_scheduled == 3
-    assert int((got.job_state == abi.JOB_FAILED).sum()) == 1
+    rc.resolution_rounding_blocks_a_feasible_node(emu_round)
 
 
 @pytest.mark.parametrize("seed", [0, 5])
@@ -177,133 +121,30 @@ def test_exact_mode_forced_on_aligned_rounds(seed):
 
 
 def test_more_classes_than_the_shared_memory_table_holds():
-    r = synth.many_classes_round()
-    got, _ = assert_parity(r.to_input(), r.name)
-    assert got.out.num_result_scheduled > 0
+    rc.more_classes_than_the_shared_memory_table_holds(emu_round)
 
 
 def test_time_budget_aborts_the_round_and_leaves_the_snapshot_runnable():
-    """armada_round_run_deadline: a budget that cannot be met returns ARMADA_E_DEADLINE (the reference's
-    cancelled context, scheduling_algo.go:115-118), download is refused, and the same handle still
-    schedules the uploaded snapshot afterwards — bit-exact.  (Emulated kernel build: no GPU needed.)"""
-    r = synth.random_round(3, n_nodes=50, n_jobs=300, n_running=60)
-    inp = r.to_input()
-    dev = emu_lib.emu_round()
-    dev.upload(inp)
-    with pytest.raises(abi.ArmadaError) as ei:
-        dev.run(budget_ns=1)
-    assert ei.value.status == abi.E_DEADLINE
-    with pytest.raises(abi.ArmadaError) as ei:
-        dev.download()
-    assert ei.value.status == abi.E_STATE
-    dev.run(budget_ns=60_000_000_000)
-    assert not dev.download().diff(oracle_lib.round_schedule(inp))
-    dev.close()
-
-
-def _dry_run_case(r, gangs_as_jobs, lib):
-    """gangs_as_jobs: lists of job indices; the product takes the jobs' classes."""
-    from armada_b200.scheduler import DeviceNodeDb
-    inp = r.to_input()
-    jc = np.asarray(r.job_class).astype(np.int64)
-    odb = oracle_lib.OracleNodeDb(inp)
-    want_ok, want_nodes = [], []
-    for g in gangs_as_jobs:
-        ok, nodes = odb.dry_run(g)
-        want_ok.append(ok)
-        want_nodes.append(nodes)
-    with DeviceNodeDb(inp, 0, lib=lib) as db:
-        got_ok, got_nodes = db.schedule_many([[int(jc[j]) for j in g] for g in gangs_as_jobs])
-        # armada_nodedb_select_nodes: the single-job form gives the same nodes as gangs of one
-        singles = [g for g in gangs_as_jobs if len(g) == 1]
-        sel = db.select_nodes([int(jc[g[0]]) for g in singles])
-        for g, n in zip(singles, sel):
-            ok, nodes = odb.dry_run(g)
-            assert (n != abi.NONE) == ok and (not ok or n == nodes[0])
-    assert list(got_ok) == want_ok
-    for g, (a, b) in enumerate(zip(got_nodes, want_nodes)):
-        assert (a == b).all(), f"gang {g}: {a} vs {b}"
-    return want_ok
+    rc.time_budget(emu_lib.emu_round, synth.random_round(3, n_nodes=50, n_jobs=300, n_running=60).to_input(), budget_ns=1)
 
 
 @pytest.mark.parametrize("seed,unaligned", [(0, False), (1, True), (2, True), (3, False)])
 def test_dry_run_nodedb_matches_the_oracle(seed, unaligned):
-    """armada_nodedb_schedule_many (SubmitChecker's ScheduleManyWithTxn + Abort on an empty cluster,
-    submitcheck.go:302-422): single jobs and gangs of every class, including gangs too big for the
-    cluster, against the oracle's NodeDb — same verdicts, same nodes."""
-    r = synth.random_round(seed, n_nodes=30 + 7 * seed, n_jobs=200, n_running=0, gangs=False, unaligned=unaligned, away=(seed == 1))
-    rng = np.random.default_rng(seed)
-    J = len(np.asarray(r.job_class))
-    gangs = [[int(j)] for j in rng.choice(J, 40, replace=False)]
-    for _ in range(12):
-        size = int(rng.integers(2, 150))
-        j0 = int(rng.integers(0, J))
-        cls = np.asarray(r.job_class)[j0]
-        same = np.nonzero(np.asarray(r.job_class) == cls)[0]
-        gangs.append([int(same[i % len(same)]) for i in range(size)] if len(same) >= 1 else [j0])
-    # the oracle's jobs must be distinct inside one gang
-    gangs = [list(dict.fromkeys(g)) for g in gangs]
-    oks = _dry_run_case(r, gangs, emu_lib.load())
-    assert any(oks)
+    rc.dry_run_nodedb_matches_the_oracle(emu_nodedb, seed, unaligned, n_nodes=30 + 7 * seed, n_jobs=200, n_singles=40, n_gangs=12, max_gang=150)
 
 
 def test_dry_run_nodedb_resolution_rounding():
-    """The rounded index key can hide a node from the iterator even on an empty cluster: 20 cpu on a
-    32-cpu node with a 17-cpu index resolution (rounded 17 < 20) is unschedulable in the reference."""
-    r = synth.rounding_round()
-    r.class_request = np.stack([synth.rl(16, 128), synth.rl(20, 128)])
-    r.class_pc = np.zeros(2)
-    r.class_static_row = np.zeros(2)
-    r.job_class = np.array([0, 0, 1, 1])
-    oks = _dry_run_case(r, [[0], [2], [0, 1], [3]], emu_lib.load())
-    assert oks == [True, False, True, False]
+    rc.dry_run_nodedb_resolution_rounding(emu_nodedb)
 
 
 @pytest.mark.parametrize("seed", [2, 4, 10])
 def test_snapshot_construction_on_the_device(seed):
-    """NULL queue_allocated_by_pc / queue_constrained_demand: the library derives the queue accounting
-    from the job arrays (calculateJobSchedulingInfo + constructSchedulingContext,
-    scheduling_algo.go:522-632,664-676) — on the device in the product (k_snapshot_*), restated in the
-    oracle; without per-queue limits that equals what the host-side generator passes explicitly."""
-    limits = seed == 4
-    r = synth.random_round(seed, n_nodes=50, n_jobs=350, n_running=100, protected_fraction=0.5, queue_limits=limits)
-    inp = r.to_input()
-    explicit = oracle_lib.round_schedule(inp)
-    inp.queue_allocated_by_pc = None
-    inp.queue_constrained_demand = None
-    want = oracle_lib.round_schedule(inp)
-    got = emu_round(inp)
-    assert not got.diff(want)
-    if not limits:
-        assert not want.diff(explicit)
-
-
-def _excluded_nodes_properties(inp, want):
-    """queue_scheduler_test.go:656-676: for a single job that could not be scheduled the excluded nodes
-    add up to the number of nodes; jobs that were never attempted (or did not fail) report nothing."""
-    ex = np.asarray(want.job_excluded_nodes)
-    st = np.asarray(want.job_state)
-    gang = np.ctypeslib.as_array(inp.job_gang, (inp.num_jobs,))
-    tot = ex.sum(axis=1)
-    assert (tot[(st != abi.JOB_FAILED) | (gang != abi.NONE)] == 0).all()
-    attempted = tot > 0
-    assert (tot[attempted] == inp.num_nodes).all()
-    return int(attempted.sum())
+    rc.snapshot_construction(emu_round, seed)
 
 
 @pytest.mark.parametrize("seed", range(8))
 def test_excluded_nodes_by_reason_kind(seed, lane_order):
-    """collect_excluded_nodes: PodSchedulingContext.NumExcludedNodesByReason of the jobs that fail, by
-    reason kind (node type / taints+labels / resources on a reached node / never reached), identical to
-    the oracle's restatement of nodedb.go:445-480,605-640,786-797,1102-1117."""
-    r = synth.random_round(700 + seed, n_nodes=40 + 7 * seed, n_queues=4, n_jobs=600, n_running=100 if seed % 2 else 0, gangs=seed % 3 == 0,
-                           priorities=seed % 2 == 1, unaligned=seed >= 6)
-    inp = r.to_input()
-    inp.collect_excluded_nodes = 1
-    want = oracle_lib.round_schedule(inp)
-    got = emu_round(inp)
-    assert not got.diff(want)
-    assert _excluded_nodes_properties(inp, want) > 0 or seed in (0,)
+    rc.excluded_nodes_by_reason_kind(emu_round, seed, unaligned=seed >= 6)
 
 
 def test_excluded_nodes_on_the_reference_tables():
@@ -312,13 +153,13 @@ def test_excluded_nodes_on_the_reference_tables():
 
     def schedule(inp):
         inp.collect_excluded_nodes = 1
-        got = _emu_round_or_skip(inp)  # (compares every array, job_excluded_nodes included, with the oracle)
-        seen.append(_excluded_nodes_properties(inp, got))
+        got = rc.round_or_skip(emu_round, inp)  # (compares every array, job_excluded_nodes included, with the oracle)
+        seen.append(rc.excluded_nodes_properties(inp, got))
         return got
 
-    for name in sorted(QS.keys()):
+    for name in sorted(rc.QS.keys()):
         try:
-            gt.run_queue_scheduler_case(QS[name], schedule)
+            gt.run_queue_scheduler_case(rc.QS[name], schedule)
         except gt.UnsupportedCase:
             continue
     assert sum(seen) > 0
@@ -351,34 +192,21 @@ def test_excluded_nodes_static_and_resource_kinds(seed, lane_order):
     r.node_static_class, r.static_match, r.num_static_classes = sc, sm2, new + 1
     inp = r.to_input()
     inp.collect_excluded_nodes = 1
-    want = oracle_lib.round_schedule(inp)
-    got = emu_round(inp)
-    assert not got.diff(want)
-    assert _excluded_nodes_properties(inp, want) > 0
+    _, want = assert_parity(inp, r.name)
+    assert rc.excluded_nodes_properties(inp, want) > 0
     ex = np.asarray(want.job_excluded_nodes)
     assert ex[:, abi.EXCL_STATIC].sum() > 0
 
 
 # ---- gang node uniformity + floating resources (gang_scheduler.go:143,154-223) ----------------------
-import gang_cases  # noqa: E402
-
-
 @pytest.mark.parametrize("name", sorted(gang_cases.GANG.keys()))
 def test_reference_gang_scheduler_table(name):
-    """TestGangScheduler (gang_scheduler_test.go:33-760) through the kernel: node-uniformity search, floating
-    resources, round / queue limits, the resolution-rounding case."""
-    b, tc, gangs = gang_cases.gang_case_round(name)
-    got, _ = assert_parity(b.input, name)
-    gang_cases.check_gang_case(b, tc, gangs, got)
+    rc.gang_scheduler_table(emu_round, name)
 
 
 @pytest.mark.parametrize("seed", range(8))
 def test_uniformity_and_floating_rounds(seed, lane_order):
-    got, want = assert_parity(gang_cases.uniformity_round(seed).input, f"uniformity round {seed}")
-    if seed == 1:  # the generator reaches every new outcome
-        reasons = set(int(x) for x in want.job_reason)
-        assert {abi.REASON_UNIFORMITY_LABEL_NOT_INDEXED, abi.REASON_NO_NODES_WITH_UNIFORMITY_LABEL, abi.REASON_GANG_FITS_NO_UNIFORMITY_VALUE,
-                abi.REASON_FLOATING_RESOURCES} <= reasons
+    rc.uniformity_and_floating_round(emu_round, seed)
 
 
 @pytest.mark.parametrize("seed", [20, 21, 22])
@@ -390,14 +218,9 @@ def test_uniformity_rounds_without_floating_resources_keep_the_batch_pipeline():
     got, _ = assert_parity(gang_cases.uniformity_round(30, n_nodes=80, n_jobs=600, floating=False).input, "uniformity, no floating")
 
 
-import order_cases  # noqa: E402
-
-
 @pytest.mark.parametrize("name", sorted(order_cases.CASES))
 def test_job_priority_comparer(name):
-    b, expected = order_cases.comparison_round(name)
-    got, _ = assert_parity(b.input, name)
-    order_cases.check_order(b, expected, got)
+    rc.job_priority_comparer(emu_round, name)
 
 
 def test_presorted_job_order_fast_path_equals_the_general_path(monkeypatch):
@@ -445,9 +268,7 @@ def test_uniformity_rounds_with_large_and_running_gangs(seed):
 def test_dry_run_nodedb_ignores_floating_resources_in_the_node_fit():
     """SubmitChecker's NodeDb with a floating resource in the factory: a job's floating request is no part of the node
     fit (KubernetesResourceRequirements) — oracle and device agree, and the job fits where its cpu / memory do."""
-    from armada_b200.scheduler import DeviceNodeDb
-
-    class _R:  # what _dry_run_case needs of a round
+    class _R:  # what dry_run_case needs of a round
         def __init__(self, b):
             self.b, self.job_class = b, b.job_class
 
@@ -462,7 +283,7 @@ def test_dry_run_nodedb_ignores_floating_resources_in_the_node_fit():
     with_lic = [j for j in range(J) if "licences" in b.jobs[j].requests and b.jobs[j].node is None]
     assert with_lic
     gangs = [[j] for j in with_lic[:10]] + [[j] for j in range(J) if b.jobs[j].node is None][:10]
-    oks = _dry_run_case(_R(b), gangs, emu_lib.load())
+    oks = rc.dry_run_case(emu_nodedb, _R(b), gangs)
     assert all(oks[: len(with_lic[:10])])  # 1–16 cpu on 32-cpu nodes of an empty cluster: every one fits
 
 

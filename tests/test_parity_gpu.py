@@ -1,15 +1,19 @@
 """Parity tests proper: the CUDA path (through the C ABI, host buffers in/out) against the CPU
 oracle on the same inputs — bit-exact on every output array (job outcomes, nodes, priorities,
 methods, reasons, final NodeDb allocatable vectors, per-queue accounting, fair-share doubles,
-counters).  Run on an H100: pytest -m gpu."""
+counters).  The bodies shared with the emulator module are in tests/round_cases.py.  Run on an
+H100: pytest -m gpu."""
 import numpy as np
 import pytest
 
+import gang_cases
 import go_tables as gt
 import oracle_lib
+import order_cases
+import round_cases as rc
 import shape_cases
 from armada_b200 import abi, synth
-from armada_b200.scheduler import DeviceRound
+from armada_b200.scheduler import DeviceNodeDb, DeviceRound
 from shape_cases import Case, compare_key  # noqa: F401  (fixture)
 
 pytestmark = pytest.mark.gpu
@@ -29,62 +33,34 @@ def cuda_round(inp):
 
 
 def assert_parity(inp, label=""):
-    want = oracle_lib.round_schedule(inp)
-    got = cuda_round(inp)
-    bad = got.diff(want)
-    assert not bad, f"{label}: CUDA != oracle:\n  " + "\n  ".join(bad)
-    return got, want
+    return rc.assert_parity(cuda_round, inp, label)
 
 
 @pytest.mark.parametrize("seed", range(24))
 def test_random_rounds(seed):
-    r = synth.random_round(
-        seed,
-        away=(seed % 4 == 1),
-        round_limit=(seed % 6 == 3),
-        queue_limits=(seed % 6 == 4),
-        protected_fraction=0.5 if seed % 3 == 2 else 0.0,
-        lookback=40 if seed % 5 == 1 else 0,
-        n_nodes=40 + 13 * (seed % 7),
-        n_jobs=300 + 50 * (seed % 5),
-        n_running=80 + 20 * (seed % 4),
-    )
-    got, _ = assert_parity(r.to_input(), r.name)
-    assert got.stats.gpu_launches > 0
+    rc.random_rounds(cuda_round, seed)
 
 
 @pytest.mark.parametrize("seed", range(100, 108))
 def test_random_rounds_many_nodes(seed):
     # > 1 tile group (N > 4096) so every tree level is exercised
-    r = synth.random_round(seed, n_nodes=5000 + 700 * (seed % 3), n_queues=9, n_jobs=6000, n_running=3000,
-                           protected_fraction=0.5 if seed % 2 else 0.0)
-    assert_parity(r.to_input(), r.name)
+    rc.random_rounds_many_nodes(cuda_round, seed, n_nodes=5000 + 700 * (seed % 3), n_jobs=6000, n_running=3000)
 
 
 @pytest.mark.parametrize("name,scale", [("C2", 0.02), ("C3", 0.004), ("C4", 0.006), ("C5", 0.004), ("C3", 0.05), ("C5", 0.03)])
 def test_scaled_configs(name, scale):
-    r = synth.scaled(name, scale)
-    got, want = assert_parity(r.to_input(), f"{name}@{scale}")
-    assert got.out.num_result_scheduled == want.out.num_result_scheduled
+    rc.scaled_config(cuda_round, name, scale)
 
 
 @pytest.mark.parametrize("n_nodes", [7, 401, 5000])
 def test_runs_of_known_unschedulable_jobs(n_nodes):
-    r = synth.unfeasible_runs_round(n_nodes)
-    got, want = assert_parity(r.to_input(), r.name)
-    assert got.out.num_result_scheduled == want.out.num_result_scheduled == 11 + 40
+    rc.runs_of_known_unschedulable_jobs(cuda_round, n_nodes)
 
 
 @pytest.mark.parametrize("seed,indexed", [(400, [synth.CPU, synth.MEM]), (401, [synth.CPU]), (402, [synth.MEM, synth.GPU]),
                                           (403, [synth.CPU, synth.MEM])])
 def test_partly_indexed_resources(seed, indexed):
-    """indexedResources ⊂ resources: no SWAR shortcuts, the assignment table keeps rows beside the keys."""
-    batchy = seed != 403
-    r = synth.random_round(seed, n_nodes=120, n_queues=6, n_jobs=900, n_running=0 if batchy else 200, gangs=not batchy, priorities=not batchy)
-    r.indexed = indexed
-    got, _ = assert_parity(r.to_input(), f"{r.name} indexed={indexed}")
-    if batchy:
-        assert int(got.stats.phase_cycles[4]) > 0
+    rc.partly_indexed_resources(cuda_round, seed, indexed)
 
 
 def test_batch_mode_covers_the_plain_iterations_and_is_deterministic():
@@ -113,38 +89,14 @@ def test_c1_simulator_config():
     assert got.out.num_result_scheduled == 1000
 
 
-PQS = gt.load_cases("preempting_queue_scheduler")
-QS = gt.load_cases("queue_scheduler")
-
-
-def _cuda_round_or_skip(inp):
-    try:
-        got = cuda_round(inp)
-    except abi.ArmadaError as e:
-        if e.status == abi.E_UNSUPPORTED:
-            raise gt.UnsupportedCase(str(e))
-        raise
-    want = oracle_lib.round_schedule(inp)
-    bad = got.diff(want)
-    assert not bad, "CUDA != oracle:\n  " + "\n  ".join(bad)
-    return got
-
-
-@pytest.mark.parametrize("name", sorted(PQS.keys()))
+@pytest.mark.parametrize("name", sorted(rc.PQS.keys()))
 def test_reference_pqs_tables_on_device(name):
-    """The reference's own TestPreemptingQueueScheduler scenarios, driven through the CUDA path."""
-    try:
-        gt.run_pqs_case(PQS[name], _cuda_round_or_skip)
-    except gt.UnsupportedCase as e:
-        pytest.skip(f"outside device domain / not modelled: {e}")
+    rc.reference_table(cuda_round, gt.run_pqs_case, rc.PQS[name])
 
 
-@pytest.mark.parametrize("name", sorted(QS.keys()))
+@pytest.mark.parametrize("name", sorted(rc.QS.keys()))
 def test_reference_queue_scheduler_tables_on_device(name):
-    try:
-        gt.run_queue_scheduler_case(QS[name], _cuda_round_or_skip)
-    except gt.UnsupportedCase as e:
-        pytest.skip(f"outside device domain / not modelled: {e}")
+    rc.reference_table(cuda_round, gt.run_queue_scheduler_case, rc.QS[name])
 
 
 def test_unsupported_input_fails_loudly():
@@ -158,14 +110,7 @@ def test_unsupported_input_fails_loudly():
 
 @pytest.mark.parametrize("seed", range(12))
 def test_exact_mode_unaligned_rounds(seed):
-    """The reference's default index resolutions (config/scheduler/config.yaml:116-124: cpu 100m, memory
-    100Mi) with 250m / 4Gi-style requests, node sizes that are not multiples of them, allocatable <
-    total, NodeFactory index order != node-id order, classes matching several node types: exact mode
-    (literal ordered walks, nodeiteration.go:318-382) — no E_UNSUPPORTED, bit-exact."""
-    r = synth.random_round(seed, away=(seed % 4 == 1), n_nodes=40 + 13 * (seed % 7), n_jobs=300 + 50 * (seed % 5),
-                           n_running=80 + 20 * (seed % 4), protected_fraction=0.5 if seed % 3 == 2 else 0.0,
-                           round_limit=(seed % 6 == 3), queue_limits=(seed % 6 == 4), lookback=40 if seed % 5 == 1 else 0, unaligned=True)
-    assert_parity(r.to_input(), r.name)
+    rc.exact_mode_unaligned_round(cuda_round, seed)
 
 
 def test_exact_mode_many_nodes():
@@ -174,9 +119,7 @@ def test_exact_mode_many_nodes():
 
 
 def test_exact_mode_resolution_rounding_blocks_a_feasible_node():
-    """gang_scheduler_test.go:244-262: the rounded index key hides a node that would fit."""
-    got, want = assert_parity(synth.rounding_round().to_input(), "rounding")
-    assert got.out.num_result_scheduled == want.out.num_result_scheduled == 3
+    rc.resolution_rounding_blocks_a_feasible_node(cuda_round)
 
 
 @pytest.mark.parametrize("name", ["C2", "C3", "C4"])
@@ -226,66 +169,22 @@ def test_full_size_properties():
     assert (qa == a.queue_allocated).all()
 
 
-def _dry_run_case(r, gangs_as_jobs):
-    from armada_b200.scheduler import DeviceNodeDb
-    inp = r.to_input()
-    jc = np.asarray(r.job_class).astype(np.int64)
-    odb = oracle_lib.OracleNodeDb(inp)
-    want = [odb.dry_run(g) for g in gangs_as_jobs]
-    with DeviceNodeDb(inp, 0) as db:
-        got_ok, got_nodes = db.schedule_many([[int(jc[j]) for j in g] for g in gangs_as_jobs])
-    assert list(got_ok) == [w[0] for w in want]
-    for g, (a, w) in enumerate(zip(got_nodes, want)):
-        assert (a == w[1]).all(), f"gang {g}: {a} vs {w[1]}"
-    return [w[0] for w in want]
-
-
 @pytest.mark.parametrize("seed,unaligned,n_nodes", [(0, False, 60), (1, True, 80), (2, True, 2500), (3, False, 5000)])
 def test_dry_run_nodedb_matches_the_oracle(seed, unaligned, n_nodes):
-    """armada_nodedb_schedule_many — SubmitChecker's ScheduleManyWithTxn + Abort on an empty cluster
-    (submitcheck.go:302-422) — for a batch of single jobs and gangs in one launch: the oracle's
-    verdicts and nodes."""
-    r = synth.random_round(seed, n_nodes=n_nodes, n_jobs=400, n_running=0, gangs=False, unaligned=unaligned, away=(seed == 1))
-    rng = np.random.default_rng(seed)
-    J = len(np.asarray(r.job_class))
-    gangs = [[int(j)] for j in rng.choice(J, 120, replace=False)]
-    for _ in range(30):
-        size = int(rng.integers(2, 200))
-        cls = np.asarray(r.job_class)[int(rng.integers(0, J))]
-        same = np.nonzero(np.asarray(r.job_class) == cls)[0]
-        gangs.append(list(dict.fromkeys(int(same[i % len(same)]) for i in range(size))))
-    assert any(_dry_run_case(r, gangs))
+    rc.dry_run_nodedb_matches_the_oracle(DeviceNodeDb, seed, unaligned, n_nodes, n_jobs=400, n_singles=120, n_gangs=30, max_gang=200)
 
 
 def test_dry_run_nodedb_resolution_rounding():
-    r = synth.rounding_round()
-    r.class_request = np.stack([synth.rl(16, 128), synth.rl(20, 128)])
-    r.class_pc = np.zeros(2)
-    r.class_static_row = np.zeros(2)
-    r.job_class = np.array([0, 0, 1, 1])
-    assert _dry_run_case(r, [[0], [2], [0, 1], [3]]) == [True, False, True, False]
+    rc.dry_run_nodedb_resolution_rounding(DeviceNodeDb)
 
 
 def test_more_classes_than_the_shared_memory_table_holds():
-    r = synth.many_classes_round(n_nodes=600, n_jobs=12000)
-    assert_parity(r.to_input(), r.name)
+    rc.more_classes_than_the_shared_memory_table_holds(cuda_round, n_nodes=600, n_jobs=12000)
 
 
 @pytest.mark.parametrize("seed", [2, 4, 10])
 def test_snapshot_construction_on_the_device(seed):
-    """NULL queue_allocated_by_pc / queue_constrained_demand: k_snapshot_jobs / k_snapshot_queues derive
-    the queue accounting from the job arrays (scheduling_algo.go:522-632,664-676)."""
-    limits = seed == 4
-    r = synth.random_round(seed, n_nodes=50, n_jobs=350, n_running=100, protected_fraction=0.5, queue_limits=limits)
-    inp = r.to_input()
-    explicit = oracle_lib.round_schedule(inp)
-    inp.queue_allocated_by_pc = None
-    inp.queue_constrained_demand = None
-    want = oracle_lib.round_schedule(inp)
-    got = cuda_round(inp)
-    assert not got.diff(want)
-    if not limits:
-        assert not want.diff(explicit)
+    rc.snapshot_construction(cuda_round, seed)
 
 
 def test_snapshot_construction_at_c5_scale():
@@ -297,20 +196,8 @@ def test_snapshot_construction_at_c5_scale():
 
 
 def test_time_budget_aborts_the_round_and_leaves_the_snapshot_runnable():
-    """armada_round_run_deadline on the device (%globaltimer): a budget that cannot be met returns
-    ARMADA_E_DEADLINE, download is refused, the same handle then schedules the snapshot bit-exactly."""
-    r = synth.scaled("C3", 0.05)
-    inp = r.to_input()
-    with DeviceRound(0) as dev:
-        dev.upload(inp)
-        with pytest.raises(abi.ArmadaError) as ei:
-            dev.run(budget_ns=1000)
-        assert ei.value.status == abi.E_DEADLINE
-        with pytest.raises(abi.ArmadaError) as ei:
-            dev.download()
-        assert ei.value.status == abi.E_STATE
-        dev.run(budget_ns=60_000_000_000)
-        assert not dev.download().diff(oracle_lib.round_schedule(inp))
+    """The budget is measured on the device (%globaltimer)."""
+    rc.time_budget(DeviceRound, synth.scaled("C3", 0.05).to_input(), budget_ns=1000)
 
 
 @pytest.mark.parametrize("nodes,queues,jobs,seed", [(60, 4, 1500, 1), (250, 6, 5000, 3), (3000, 16, 40000, 5)])
@@ -340,18 +227,7 @@ def test_rounds_of_different_handles_run_concurrently_and_stay_exact():
 
 @pytest.mark.parametrize("seed", range(6))
 def test_excluded_nodes_by_reason_kind(seed):
-    """collect_excluded_nodes: NumExcludedNodesByReason of the failed single jobs by reason kind, equal to
-    the oracle's; the kinds of an attempted job add up to the number of nodes
-    (queue_scheduler_test.go:656-676)."""
-    r = synth.random_round(700 + seed, n_nodes=40 + 7 * seed, n_queues=4, n_jobs=600, n_running=100 if seed % 2 else 0, gangs=seed % 3 == 0,
-                           priorities=seed % 2 == 1, unaligned=seed >= 4)
-    inp = r.to_input()
-    inp.collect_excluded_nodes = 1
-    got, want = assert_parity(inp, r.name)
-    ex = np.asarray(got.job_excluded_nodes)
-    tot = ex.sum(axis=1)
-    assert (tot[np.asarray(got.job_state) != abi.JOB_FAILED] == 0).all()
-    assert (tot[tot > 0] == inp.num_nodes).all() and (tot > 0).any()
+    rc.excluded_nodes_by_reason_kind(cuda_round, seed, unaligned=seed >= 4)
 
 
 def test_excluded_nodes_at_c3_scale():
@@ -359,24 +235,18 @@ def test_excluded_nodes_at_c3_scale():
     inp = r.to_input()
     inp.collect_excluded_nodes = 1
     got, _ = assert_parity(inp, "C3@0.05 with excluded-node kinds")
-    tot = np.asarray(got.job_excluded_nodes).sum(axis=1)
-    assert (tot[tot > 0] == inp.num_nodes).all() and (tot > 0).any()
+    assert rc.excluded_nodes_properties(inp, got) > 0
 
 
 # ---- gang node uniformity + floating resources (gang_scheduler.go:143,154-223) ----------------------
-import gang_cases  # noqa: E402
-
-
 @pytest.mark.parametrize("name", sorted(gang_cases.GANG.keys()))
 def test_reference_gang_scheduler_table_on_device(name):
-    b, tc, gangs = gang_cases.gang_case_round(name)
-    got, _ = assert_parity(b.input, name)
-    gang_cases.check_gang_case(b, tc, gangs, got)
+    rc.gang_scheduler_table(cuda_round, name)
 
 
 @pytest.mark.parametrize("seed", range(10))
 def test_uniformity_and_floating_rounds(seed):
-    assert_parity(gang_cases.uniformity_round(seed).input, f"uniformity round {seed}")
+    rc.uniformity_and_floating_round(cuda_round, seed)
 
 
 @pytest.mark.parametrize("seed,unaligned,floating", [(40, False, False), (41, True, True), (42, False, True)])
@@ -386,14 +256,9 @@ def test_uniformity_rounds_at_scale(seed, unaligned, floating):
     assert int(want.out.num_result_scheduled) > 1000
 
 
-import order_cases  # noqa: E402
-
-
 @pytest.mark.parametrize("name", sorted(order_cases.CASES))
 def test_job_priority_comparer_on_device(name):
-    b, expected = order_cases.comparison_round(name)
-    got, _ = assert_parity(b.input, name)
-    order_cases.check_order(b, expected, got)
+    rc.job_priority_comparer(cuda_round, name)
 
 
 # ---- every resource count and key layout (tests/shape_cases.py), and the emulator's knob tests on the device ----

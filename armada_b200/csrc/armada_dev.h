@@ -26,6 +26,26 @@
 #define ARMADA_DEV_MAX_SLOTS 22  // best-fit index slots: 2 per owning index warp (11 owners; batch mode keeps both in registers)
 #define ARMADA_DEV_VARIANTS (1 + ARMADA_MAX_AWAY)  // home + away node types per class
 
+// Slots of DevPtrs::stats: counters summed over the schedule passes of a round (k_reset zeroes them; the host
+// reads them into ArmadaRoundStats and the ARMADA_PRINT_STATS lines).  A group of n slots starts at its base.
+enum StatSlot {
+  STAT_ITERS = 0,       // loop iterations
+  STAT_PROBES = 1,
+  STAT_PLACEMENTS = 2,
+  STAT_FAIR = 3,        // fair-preemption scans
+  STAT_RESCANS = 4,     // ArmadaRoundStats::tree_rescans
+  STAT_KERNEL = 5,      // control-warp cycles: the whole kernel
+  STAT_STARTUP = 6,     // … before the loop
+  STAT_RUNS = 7,        // … in pipeline runs
+  STAT_PROF = 8,        // [8] ArmadaRoundStats::phase_cycles
+  STAT_BT_CYC = 16,     // [8] ArmadaRoundStats::batch_cycles
+  STAT_BT_DBG = 24,     // [8] ArmadaRoundStats::batch_debug
+  STAT_TL = 32,         // [8] control-warp timeline
+  STAT_GL = 40,         // [8] general-loop timeline
+  STAT_GATE = 48,       // [2] level-0 miss gate probes: run, skipped
+  STAT_COUNT = 50,
+};
+
 struct DevCfg {  // small POD, lives in global memory, hot parts copied to smem
   int32_t D, R, PL, PC, Q, C, T, S, rows;
   uint32_t N, J, G;
@@ -163,7 +183,6 @@ struct DevPtrs {
   uint32_t* bt_pos;                // stream position of the item
   uint32_t* bt_rank;               // merged position
   uint2* bt_seq;                   // merged sequence: {job, class}
-  uint32_t* bt_node;               // (unused)
   int64_t* bt_asum;                // [2][Q][MAX_RESOURCES] requests of every queue's items below the horizon, per batch buffer
   uint32_t* bt_card;               // [2][Q * bt_wq] members of the item (1 = single job, > 1 = a simple gang)
   uint4* bt_item;                  // [2][Q * bt_wq] merged order: {queue, stream position of the item's last job, members, 0}
@@ -177,8 +196,6 @@ struct DevPtrs {
   const uint32_t* row_type_excl;   // [rows] nodes of the node types the row does not match (NodeTypesMatchingJob)
   uint32_t* undo_log;              // [5 * J] txn undo records
   // fair preemption scratch
-  int64_t* fp_avail;               // [D][N]
-  uint32_t* fp_epoch;              // [N]
   uint32_t* fp_head;               // [N] most recent visited evicted index on the node
   uint32_t* fp_next;               // [J] chain by evicted index
   uint32_t* nl_start;              // [N+1] node n's evicted jobs = nl_item[nl_start[n] .. nl_start[n+1]) (built after the indices are assigned)
@@ -189,7 +206,6 @@ struct DevPtrs {
   uint32_t* bver;                  // [ceil(N/256)] changes of any node of the 256-node block (sum of its nver)
   uint32_t* fc_bver;               // [8][ceil(N/256)] bver the block's cached maximum was computed at
   unsigned long long* fc_bmax;     // [8][ceil(N/256)] largest (trigger + 1) << 32 | node of the block, 0 = none
-  uint8_t* fp_bad;                 // [N] static requirements not met (valid when epoch matches)
   // ---- queue / sctx state persisted between kernels ----
   int64_t* q_alloc;                // [Q][D]
   int64_t* q_alloc_pc;             // [Q][PC][D]
@@ -200,5 +216,5 @@ struct DevPtrs {
   int64_t* s_counts;               // [8]: 0 numScheduledJobs 1 numScheduledGangs 2 numEvictedJobs
                                    //      3 termination(pass1) 4 global tokens (double bits)
   uint32_t* dbg_host;              // [64] host-mapped: written by the device watchdog before it traps
-  unsigned long long* stats;       // [8]: loop iters, probes, placements, fair scans, rescans
+  unsigned long long* stats;       // [STAT_COUNT] counters of the round's schedule passes (StatSlot)
 };

@@ -14,12 +14,12 @@
 //   * data-parallel phases (bind running jobs, both evictors, gang completion, accounting,
 //     result algebra) are grid-wide kernels over the job SoA with int64 atomics on the node SoA;
 //   * evicted jobs are ranked per queue with an LSD radix sort on (queue, order-rank) keys;
-//   * the inherently sequential QueueScheduler loop runs in ONE persistent CTA: warp 0 is the
-//     control warp (DRF arg-min over queues by warp reduction, gang iterator, constraints,
-//     bind), warps 0..31 jointly maintain per-(job shape, priority level) best-fit tournament
-//     trees in shared memory whose leaves are coalesced 128-node tile scans of the HBM/L2
-//     resident node SoA with redux.sync arg-min on a packed 64-bit (resources…, node-id) key.
-//     A probe is a root read; a bind re-scans one tile per affected tree.
+//   * the inherently sequential QueueScheduler loop runs in ONE persistent CTA of 16 warps
+//     (armada_pass.inc, DESIGN §5.1–5.2): warp 15 is the control warp (DRF arg-min over queues,
+//     gang iterator, constraints, bind); the 15 index warps keep the best-fit index — all nodes
+//     radix-sorted by their packed (resources…, node-id) key in HBM, plus a 32-entry sorted window
+//     of the smallest feasible keys per (job class × node-type variant) in shared memory.
+//     A probe reads a window head; a bind posts the node's new row to the index warps.
 //   Tensor cores are not used: this is integer compare/select work.
 #ifdef ARMADA_EMU
 #include "cuda_emu.h"  // tools/simt_emu: deterministic CPU SIMT emulator (dev/test tooling only)
@@ -116,10 +116,9 @@ __global__ void k_reset(DevCfg c, DevPtrs P) {
     P.gang_fill[g] = 0;
     P.gang_ev[g] = 0;
   }
-  for (size_t n = i; n < c.N; n += stride) P.fp_epoch[n] = 0;
   for (size_t k = i; k < (size_t)c.C; k += stride) P.unfeasible[k] = 0;
   if (i < 16) P.counters[i] = 0;
-  if (i < 50) P.stats[i] = 0;
+  if (i < STAT_COUNT) P.stats[i] = 0;
 }
 
 // CreateAndInsertWithJobDbJobsWithTxn (nodedb.go:43-60): bind every running job at its

@@ -7,6 +7,8 @@ from __future__ import annotations
 import ctypes as C
 import os
 
+import numpy as np
+
 ABI_VERSION = 2
 MAX_RESOURCES = 8
 EXCLUDED_KINDS = 5  # ARMADA_EXCL_*: node type, static, resources (reached), implicit, disallowed
@@ -192,6 +194,25 @@ class ExcludedReason(C.Structure):
         ("count", C.c_uint32),
         ("_pad", C.c_uint32),
     ]
+
+
+def field_dtype(struct_type, name: str) -> np.dtype:
+    """The element type of pointer field `name` of a structure above, as a numpy dtype."""
+    return np.dtype(dict(struct_type._fields_)[name]._type_)
+
+
+def attach(struct, keep: list, **arrays) -> dict:
+    """Point the pointer fields of `struct` named by the keywords at their arrays.  Each array is first made
+    C-contiguous with its field's element type (declared once, in `_fields_`), so the library never reads
+    bytes as the wrong type; it is appended to `keep`, because the struct holds only raw pointers.  Returns
+    the arrays the fields point into, by field name."""
+    fields, out = dict(type(struct)._fields_), {}
+    for name, a in arrays.items():
+        a = np.ascontiguousarray(a, dtype=np.dtype(fields[name]._type_))
+        keep.append(a)
+        setattr(struct, name, a.ctypes.data_as(fields[name]))
+        out[name] = a
+    return out
 
 
 REPO_ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))

@@ -14,8 +14,8 @@ The string logic runs on the host; the device only sees dense ids and bitmaps.
 """
 from __future__ import annotations
 
-import ctypes as C
 import math
+import operator
 from dataclasses import dataclass, field
 from fractions import Fraction
 from typing import Dict, List, Optional, Sequence, Tuple
@@ -283,7 +283,12 @@ def multiply_resource(res: int, m: float) -> int:
 
 
 class RoundInputBuilder:
-    """Flattens (config, nodes, jobs, queues) into an ArmadaRoundInput.  Keeps the numpy arrays alive."""
+    """Flattens (config, nodes, jobs, queues) into an ArmadaRoundInput.  Every array the input points into is the
+    builder's attribute of the field's name and lives as long as the builder."""
+
+    # NULL unless a gang of the round has a node uniformity label / the caller gives its queued order
+    gang_uniformity_label = uniformity_value_start = class_uniformity_row = None
+    queued_start = queued_order = None
 
     def __init__(self, cfg: SchedulingConfig, nodes: Sequence[NodeSpec], jobs: Sequence[JobSpec],
                  queues: Sequence[QueueSpec], total_resources: Optional[np.ndarray] = None,
@@ -299,18 +304,32 @@ class RoundInputBuilder:
         self._keep: List[object] = []
         self.pc_names = sorted(cfg.priority_classes.keys())
         self.pc_index = {n: i for i, n in enumerate(self.pc_names)}
-        self._build(total_resources, queued_order, global_limiter_tokens)
+        self.input = abi.RoundInput()
+        self.input._keepalive = self._keep
+        self._rows: Dict[object, int] = {}  # the static bitmap rows: key -> index into row_specs
+        self.row_specs: List[Tuple[Tuple[Toleration, ...], Tuple[Tuple[str, str], ...], object]] = []
+        self._config()
+        class_meta = self._job_classes()
+        class_uniformity_row = self._uniformity_rows(class_meta)  # adds rows, so it runs before anything reads the row table
+        self._nodes()  # the row table → the label keys rows look at → the static classes
+        self._match()
+        self._jobs(class_uniformity_row)
+        self._context(total_resources, global_limiter_tokens)
+        self._queues()  # the per-queue limits are fractions of _context's total_resources
+        if queued_order is not None:
+            self._queued_order(queued_order)
 
     # -- helpers ---------------------------------------------------------------------------
-    def _arr(self, a, dtype):
-        a = np.ascontiguousarray(a, dtype=dtype)
-        self._keep.append(a)
-        return a
+    def _attach(self, **arrays):
+        vars(self).update(abi.attach(self.input, self._keep, **arrays))
 
-    def _ptr(self, a, ctype):
-        if a is None:
-            return None
-        return a.ctypes.data_as(C.POINTER(ctype))
+    def _row(self, tolerations, selector, affinity) -> int:
+        """The static row of (tolerations, node selector, affinity); a new one is appended to row_specs."""
+        key = (tuple(sorted(tolerations, key=repr)), tuple(sorted(selector.items())), affinity)
+        if key not in self._rows:
+            self._rows[key] = len(self.row_specs)
+            self.row_specs.append((tuple(tolerations), tuple(sorted(selector.items())), affinity))
+        return self._rows[key]
 
     def _node_taints(self, n: NodeSpec) -> Tuple[Taint, ...]:
         t = tuple(n.taints)
@@ -350,23 +369,20 @@ class RoundInputBuilder:
                 out.append(Toleration(key=t.key, value=t.value, effect=t.effect))
         return tuple(out)
 
-    # -- main ------------------------------------------------------------------------------
-    def _build(self, total_resources, queued_order, global_limiter_tokens):
-        cfg, f = self.cfg, self.factory
-        D = f.D
-        inp = abi.RoundInput()
+    # -- stages, in the order __init__ runs them --------------------------------------------
+    def _config(self):
+        """Resources, the node index, priorities and priority classes."""
+        cfg, f, inp = self.cfg, self.factory, self.input
         inp.abi_version = abi.ABI_VERSION
-        inp.num_resources = D
-        R = len(cfg.indexed_resources)
-        inp.num_indexed = R
+        inp.num_resources = f.D
+        inp.num_indexed = len(cfg.indexed_resources)
         for i, r in enumerate(cfg.indexed_resources):
             inp.indexed_resource[i] = f.index[r.name]
             inp.indexed_resolution[i] = f.scaled_value(r.name, r.resolution)  # makeIndexedResourceResolution
-        prios = [-1] + cfg.allowed_priorities()
-        inp.num_priorities = len(prios)
-        for i, p in enumerate(prios):
+        self.priorities = [-1] + cfg.allowed_priorities()
+        inp.num_priorities = len(self.priorities)
+        for i, p in enumerate(self.priorities):
             inp.priorities[i] = p
-        self.priorities = prios
         well_known_names = sorted(cfg.well_known_node_types.keys())
         inp.num_priority_classes = len(self.pc_names)
         for i, name in enumerate(self.pc_names):
@@ -380,32 +396,10 @@ class RoundInputBuilder:
                 # (a name without a WellKnownNodeTypes entry adds no taints here; the reference fails the away attempt that reaches it)
                 s.away_well_known[k] = well_known_names.index(a.well_known_node_type) if a.well_known_node_type in well_known_names else abi.NONE
 
-        # ---- nodes ----
-        N = len(self.nodes)
-        inp.num_nodes = N
-        node_total = np.zeros((D, N), dtype=np.int64)
-        node_alloc = np.zeros((D, N), dtype=np.int64)
-        for i, n in enumerate(self.nodes):
-            node_total[:, i] = f.from_node(n.total)
-            node_alloc[:, i] = f.from_node(n.allocatable if n.allocatable is not None else n.total)
-        ids_sorted = sorted(range(N), key=lambda i: self.nodes[i].id)
-        id_rank = np.zeros(N, dtype=np.uint32)
-        for r, i in enumerate(ids_sorted):
-            id_rank[i] = r
-        indexed_taints = None if cfg.indexed_taints is None else set(cfg.indexed_taints)
-        indexed_labels = set(cfg.indexed_node_labels)
-
-        # ---- job classes / static rows ----
-        rows: Dict[object, int] = {}
-        row_specs: List[Tuple[Tuple[Toleration, ...], Tuple[Tuple[str, str], ...], object]] = []
-
-        def row_of(tolerations, selector, affinity) -> int:
-            key = (tuple(sorted(tolerations, key=repr)), tuple(sorted(selector.items())), affinity)
-            if key not in rows:
-                rows[key] = len(row_specs)
-                row_specs.append((tuple(tolerations), tuple(sorted(selector.items())), affinity))
-            return rows[key]
-
+    def _job_classes(self) -> List[Tuple[Tuple[Toleration, ...], Dict[str, str], object, List[Tuple[Toleration, ...]]]]:
+        """Job classes with their home and away rows, and each job's class.  Returns per class its tolerations,
+        selector, affinity and per away node type the tolerations it adds, from which the uniformity rows are made."""
+        cfg, f = self.cfg, self.factory
         classes: Dict[object, int] = {}
         class_req: List[np.ndarray] = []
         class_pc: List[int] = []
@@ -422,18 +416,28 @@ class RoundInputBuilder:
                 class_req.append(req)
                 pc = cfg.priority_classes[j.priority_class]
                 class_pc.append(self.pc_index[j.priority_class])
-                class_row.append(row_of(j.tolerations, j.node_selector, j.affinity))
+                class_row.append(self._row(j.tolerations, j.node_selector, j.affinity))
                 aw = [abi.NONE] * abi.MAX_AWAY
                 extras: List[Tuple[Toleration, ...]] = []
                 for k in range(len(pc.away_node_types)):
                     extra = self._away_tolerations(pc, k, req)
                     extras.append(extra)
                     if extra:
-                        aw[k] = row_of(tuple(j.tolerations) + extra, j.node_selector, j.affinity)
+                        aw[k] = self._row(tuple(j.tolerations) + extra, j.node_selector, j.affinity)
                 class_away.append(aw)
                 class_meta.append((tuple(j.tolerations), dict(j.node_selector), j.affinity, extras))
             job_class[ji] = classes[key]
-        # ---- gang node uniformity (gang_scheduler.go:154-223): value slots per label, rows per (class, slot) ----
+        if not class_req:  # keep arrays non-empty for the C side (no jobs: no uniformity rows follow this row)
+            class_req, class_pc, class_row, class_away = [np.zeros(f.D, np.int64)], [0], [self._row((), {}, None)], [[abi.NONE] * abi.MAX_AWAY]
+        self.input.num_classes = len(class_req)
+        self._attach(class_request=np.stack(class_req), class_pc=class_pc, class_static_row=class_row, class_away_row=class_away,
+                     class_key_valid=np.ones(len(class_req)), job_class=job_class if self.jobs else [0])
+        return class_meta
+
+    def _uniformity_rows(self, class_meta) -> np.ndarray:
+        """Gang node uniformity (gang_scheduler.go:154-223): value slots per label, rows per (class, slot).  Adds
+        rows to the row table; returns the [C][V][1 + MAX_AWAY] rows for class_uniformity_row."""
+        indexed_labels = set(self.cfg.indexed_node_labels)
         uni_labels: Dict[str, int] = {}
         uni_values: List[List[str]] = []
         uni_classes: Dict[int, set] = {}
@@ -444,31 +448,42 @@ class RoundInputBuilder:
             if lab not in uni_labels:  # nodeDb.IndexedNodeLabelValues(label) minus "" (:181-190)
                 uni_labels[lab] = len(uni_values)
                 uni_values.append(sorted({self._node_labels(n)[lab] for n in self.nodes if self._node_labels(n).get(lab)}))
-            uni_classes.setdefault(uni_labels[lab], set()).add(int(job_class[ji]))
+            uni_classes.setdefault(uni_labels[lab], set()).add(int(self.job_class[ji]))
         uni_start = [0]
         for vals in uni_values:
             uni_start.append(uni_start[-1] + len(vals))
-        Vn = uni_start[-1]
-        class_uni = np.full((max(1, len(class_req)), max(1, Vn), 1 + abi.MAX_AWAY), abi.NONE, dtype=np.uint32)
+        class_uni = np.full((self.input.num_classes, max(1, uni_start[-1]), 1 + abi.MAX_AWAY), abi.NONE, dtype=np.uint32)
         for lab, li in uni_labels.items():
             for c in uni_classes.get(li, ()):
                 tol, sel, aff, extras = class_meta[c]
                 for vi, val in enumerate(uni_values[li]):
                     sel2 = dict(sel)
                     sel2[lab] = val  # jctx.AddNodeSelector
-                    class_uni[c, uni_start[li] + vi, 0] = row_of(tol, sel2, aff)
+                    class_uni[c, uni_start[li] + vi, 0] = self._row(tol, sel2, aff)
                     for k, extra in enumerate(extras):
                         if extra:
-                            class_uni[c, uni_start[li] + vi, 1 + k] = row_of(tol + extra, sel2, aff)
+                            class_uni[c, uni_start[li] + vi, 1 + k] = self._row(tol + extra, sel2, aff)
         self.uni_labels, self.uni_values, self.uni_start = uni_labels, uni_values, uni_start
-        Cn = max(1, len(class_req))
-        if not class_req:  # keep arrays non-empty for the C side
-            class_req, class_pc, class_row, class_away = [np.zeros(D, np.int64)], [0], [row_of((), {}, None)], [[abi.NONE] * abi.MAX_AWAY]
-        inp.num_classes = len(class_req)
+        return class_uni
 
+    def _nodes(self):
+        """Node resources, id ranks, static classes, node types and flags."""
+        cfg, f, inp = self.cfg, self.factory, self.input
+        N, D = len(self.nodes), f.D
+        inp.num_nodes = N
+        node_total = np.zeros((D, N), dtype=np.int64)
+        node_alloc = np.zeros((D, N), dtype=np.int64)
+        for i, n in enumerate(self.nodes):
+            node_total[:, i] = f.from_node(n.total)
+            node_alloc[:, i] = f.from_node(n.allocatable if n.allocatable is not None else n.total)
+        id_rank = np.zeros(N, dtype=np.uint32)
+        for r, i in enumerate(sorted(range(N), key=lambda i: self.nodes[i].id)):
+            id_rank[i] = r
+        indexed_taints = None if cfg.indexed_taints is None else set(cfg.indexed_taints)
+        indexed_labels = set(cfg.indexed_node_labels)
         # relevant label keys: only labels some row looks at distinguish static classes
         rel_keys = set()
-        for (_, selector, affinity) in row_specs:
+        for (_, selector, affinity) in self.row_specs:
             rel_keys.update(k for k, _ in selector)
             if affinity:
                 for term in affinity:
@@ -501,22 +516,30 @@ class RoundInputBuilder:
                 type_specs.append((ttaints, tlabels, unset))
             node_type[i] = types[tkey]
             node_flags[i] = (abi.NODE_UNSCHEDULABLE if n.unschedulable else 0) | (abi.NODE_OVERALLOCATED if n.over_allocated else 0)
-        S, T = max(1, len(static_specs)), max(1, len(type_specs))
-        inp.num_static_classes, inp.num_node_types = S, T
-        nrows = len(row_specs)
-        inp.num_static_rows = nrows
-        sw, tw = (S + 31) // 32, (T + 31) // 32
-        static_match = np.zeros((nrows, sw), dtype=np.uint32)
-        type_match = np.zeros((nrows, tw), dtype=np.uint32)
-        for r, (tolerations, selector, affinity) in enumerate(row_specs):
-            for s, (taints, labels) in enumerate(static_specs):
+        inp.num_static_classes, inp.num_node_types = max(1, len(static_specs)), max(1, len(type_specs))
+        self.static_specs, self.type_specs = static_specs, type_specs
+        self.type_keys = list(types.keys())
+        self._attach(node_index=[n.index for n in self.nodes] or [0], node_id_rank=id_rank if N else [0],
+                     node_type=node_type if N else [0], node_static_class=node_static if N else [0],
+                     node_flags=node_flags if N else [0], node_total=node_total if N else np.zeros((D, 1)),
+                     node_allocatable=node_alloc if N else np.zeros((D, 1)))
+
+    def _match(self):
+        """Per row, the static classes (static_match) and node types (type_match) its requirements admit."""
+        S, T = self.input.num_static_classes, self.input.num_node_types
+        nrows = len(self.row_specs)
+        self.input.num_static_rows = nrows
+        static_match = np.zeros((nrows, (S + 31) // 32), dtype=np.uint32)
+        type_match = np.zeros((nrows, (T + 31) // 32), dtype=np.uint32)
+        for r, (tolerations, selector, affinity) in enumerate(self.row_specs):
+            for s, (taints, labels) in enumerate(self.static_specs):
                 ok = find_untolerated(taints, tolerations) is None  # NodeTolerationRequirementsMet
                 ok = ok and all(labels.get(k) == v for k, v in selector)  # NodeSelectorRequirementsMet(node, nil)
                 if ok and affinity is not None:
                     ok = match_node_selector_terms(labels, affinity)  # NodeAffinityRequirementsMet
                 if ok:
                     static_match[r, s >> 5] |= np.uint32(1 << (s & 31))
-            for t, (ttaints, tlabels, unset) in enumerate(type_specs):
+            for t, (ttaints, tlabels, unset) in enumerate(self.type_specs):
                 ok = find_untolerated(ttaints, tolerations) is None  # TolerationRequirementsMet(nodeType)
                 if ok:
                     for k, v in selector:  # NodeSelectorRequirementsMet(type labels, unsetIndexedLabels)
@@ -529,41 +552,11 @@ class RoundInputBuilder:
                             break
                 if ok:
                     type_match[r, t >> 5] |= np.uint32(1 << (t & 31))
-        self.row_specs, self.static_specs, self.type_specs = row_specs, static_specs, type_specs
-        self.type_keys = list(types.keys())
+        self._attach(static_match=static_match, type_match=type_match)
 
-        a = self._arr
-        self.node_index = a([n.index for n in self.nodes] or [0], np.uint64)
-        self.node_id_rank = a(id_rank if N else [0], np.uint32)
-        self.node_type = a(node_type if N else [0], np.uint32)
-        self.node_static = a(node_static if N else [0], np.uint32)
-        self.node_flags = a(node_flags if N else [0], np.uint8)
-        self.node_total = a(node_total if N else np.zeros((D, 1)), np.int64)
-        self.node_alloc = a(node_alloc if N else np.zeros((D, 1)), np.int64)
-        inp.node_index = self._ptr(self.node_index, C.c_uint64)
-        inp.node_id_rank = self._ptr(self.node_id_rank, C.c_uint32)
-        inp.node_type = self._ptr(self.node_type, C.c_uint32)
-        inp.node_static_class = self._ptr(self.node_static, C.c_uint32)
-        inp.node_flags = self._ptr(self.node_flags, C.c_uint8)
-        inp.node_total = self._ptr(self.node_total, C.c_int64)
-        inp.node_allocatable = self._ptr(self.node_alloc, C.c_int64)
-
-        self.class_request = a(np.stack(class_req), np.int64)
-        self.class_pc = a(class_pc, np.uint32)
-        self.class_row = a(class_row, np.uint32)
-        self.class_away = a(class_away, np.uint32)
-        self.class_key_valid = a(np.ones(len(class_req)), np.uint8)
-        self.static_match = a(static_match, np.uint32)
-        self.type_match = a(type_match, np.uint32)
-        inp.class_request = self._ptr(self.class_request, C.c_int64)
-        inp.class_pc = self._ptr(self.class_pc, C.c_uint32)
-        inp.class_static_row = self._ptr(self.class_row, C.c_uint32)
-        inp.class_away_row = self._ptr(self.class_away, C.c_uint32)
-        inp.class_key_valid = self._ptr(self.class_key_valid, C.c_uint8)
-        inp.static_match = self._ptr(self.static_match, C.c_uint32)
-        inp.type_match = self._ptr(self.type_match, C.c_uint32)
-
-        # ---- jobs ----
+    def _jobs(self, class_uniformity_row: np.ndarray):
+        """Per-job arrays, gangs and the gangs' uniformity labels."""
+        inp = self.input
         J = len(self.jobs)
         inp.num_jobs = J
         gangs: Dict[Tuple[str, str], int] = {}
@@ -575,9 +568,8 @@ class RoundInputBuilder:
         job_qp = np.zeros(max(J, 1), dtype=np.uint32)
         job_st = np.zeros(max(J, 1), dtype=np.int64)
         job_art = np.zeros(max(J, 1), dtype=np.int64)
-        jid_sorted = sorted(range(J), key=lambda i: self.jobs[i].id)
         job_id_rank = np.zeros(max(J, 1), dtype=np.uint32)
-        for r, i in enumerate(jid_sorted):
+        for r, i in enumerate(sorted(range(J), key=lambda i: self.jobs[i].id)):
             job_id_rank[i] = r
         for ji, j in enumerate(self.jobs):
             if j.queue in self.queue_index:
@@ -596,39 +588,23 @@ class RoundInputBuilder:
             job_st[ji] = j.submit_time
             job_art[ji] = j.active_run_timestamp
         inp.num_gangs = len(gang_card)
-        self.job_class = a(job_class if J else [0], np.uint32)
-        self.job_queue = a(job_queue, np.uint32)
-        self.job_qp = a(job_qp, np.uint32)
-        self.job_st = a(job_st, np.int64)
-        self.job_id_rank = a(job_id_rank, np.uint32)
-        self.job_gang = a(job_gang, np.uint32)
-        self.job_node = a(job_node, np.uint32)
-        self.job_sap = a(job_sap, np.int32)
-        self.job_art = a(job_art, np.int64)
-        self.gang_card = a(gang_card or [0], np.uint32)
-        inp.job_class = self._ptr(self.job_class, C.c_uint32)
-        inp.job_queue = self._ptr(self.job_queue, C.c_uint32)
-        inp.job_queue_priority = self._ptr(self.job_qp, C.c_uint32)
-        inp.job_submit_time = self._ptr(self.job_st, C.c_int64)
-        inp.job_id_rank = self._ptr(self.job_id_rank, C.c_uint32)
-        inp.job_gang = self._ptr(self.job_gang, C.c_uint32)
-        inp.job_node = self._ptr(self.job_node, C.c_uint32)
-        inp.job_scheduled_at_priority = self._ptr(self.job_sap, C.c_int32)
-        inp.job_active_run_timestamp = self._ptr(self.job_art, C.c_int64)
-        inp.gang_cardinality = self._ptr(self.gang_card, C.c_uint32)
+        self._attach(job_queue=job_queue, job_queue_priority=job_qp, job_submit_time=job_st, job_id_rank=job_id_rank,
+                     job_gang=job_gang, job_node=job_node, job_scheduled_at_priority=job_sap, job_active_run_timestamp=job_art,
+                     gang_cardinality=gang_card or [0])
+        indexed_labels = set(self.cfg.indexed_node_labels)
         gang_label = np.full(max(1, len(gang_card)), abi.NONE, dtype=np.uint32)
         for ji, j in enumerate(self.jobs):
             if job_gang[ji] != abi.NONE and j.gang_node_uniformity_label:
                 lab = j.gang_node_uniformity_label
                 gang_label[job_gang[ji]] = self.uni_labels[lab] if lab in indexed_labels else abi.LABEL_NOT_INDEXED
-        self.gang_label = a(gang_label, np.uint32)
-        self.uni_start_arr = a(self.uni_start, np.uint32)
-        self.class_uni = a(class_uni, np.uint32)
         if (gang_label != abi.NONE).any():
-            inp.gang_uniformity_label = self._ptr(self.gang_label, C.c_uint32)
             inp.num_uniformity_labels = len(self.uni_values)
-            inp.uniformity_value_start = self._ptr(self.uni_start_arr, C.c_uint32)
-            inp.class_uniformity_row = self._ptr(self.class_uni, C.c_uint32)
+            self._attach(gang_uniformity_label=gang_label, uniformity_value_start=self.uni_start,
+                         class_uniformity_row=class_uniformity_row)
+
+    def _context(self, total_resources, global_limiter_tokens):
+        """Floating resources, the scheduling context's scalars, the round's limits and its rate limiter."""
+        cfg, f, inp = self.cfg, self.factory, self.input
         # floating resources (floatingresources/floating_resource_types.go:19-37)
         fmask = 0
         for fr in cfg.floating_resources:
@@ -638,12 +614,10 @@ class RoundInputBuilder:
                 inp.floating_limits_configured = 1
                 inp.floating_limit[d] = f.scaled_value(fr.name, fr.quantity)
         inp.floating_resource_mask = fmask
-
-        # ---- scheduling context scalars ----
         if total_resources is None:  # nodeDb.TotalKubernetesResources(): Σ allocatable
-            total_resources = node_alloc.sum(axis=1) if N else np.zeros(D, np.int64)
+            total_resources = self.node_allocatable.sum(axis=1) if self.nodes else np.zeros(f.D, np.int64)
         self.total_resources = np.asarray(total_resources, dtype=np.int64)
-        for d in range(D):
+        for d in range(f.D):
             inp.total_resources[d] = int(self.total_resources[d])
         mult = {}
         if cfg.drf_multipliers:
@@ -674,10 +648,11 @@ class RoundInputBuilder:
         inp.global_limiter_burst = min(cfg.maximum_scheduling_burst, 2**62)
         inp.global_limiter_tokens = float(inp.global_limiter_burst) if global_limiter_tokens is None else global_limiter_tokens
 
-        # ---- queues ----
-        Qn = len(self.queues)
-        inp.num_queues = Qn
-        PCn = len(self.pc_names)
+    def _queues(self):
+        """Per-queue weights, accounting, limits (from total_resources) and rate limiters."""
+        cfg, f = self.cfg, self.factory
+        Qn, PCn, D = len(self.queues), len(self.pc_names), f.D
+        self.input.num_queues = Qn
         qw = np.zeros(max(Qn, 1), dtype=np.float64)
         qc = np.zeros(max(Qn, 1), dtype=np.uint8)
         qa = np.zeros((max(Qn, 1), PCn, D), dtype=np.int64)
@@ -713,32 +688,33 @@ class RoundInputBuilder:
             qb[i] = min(cfg.maximum_per_queue_scheduling_burst, 2**62)
             qt[i] = float(qb[i]) if q.limiter_tokens is None else q.limiter_tokens
             qi[i] = int(math.isinf(cfg.maximum_per_queue_scheduling_rate))
-        self.qw, self.qc, self.qa, self.qd, self.qcd, self.qp = a(qw, np.float64), a(qc, np.uint8), a(qa, np.int64), a(qd, np.int64), a(qcd, np.int64), a(qp, np.int64)
-        self.qhl, self.ql, self.qt, self.qb, self.qi = a(qhl, np.uint8), a(ql, np.int64), a(qt, np.float64), a(qb, np.int64), a(qi, np.uint8)
-        inp.queue_weight = self._ptr(self.qw, C.c_double)
-        inp.queue_cordoned = self._ptr(self.qc, C.c_uint8)
-        inp.queue_allocated_by_pc = self._ptr(self.qa, C.c_int64)
-        inp.queue_demand = self._ptr(self.qd, C.c_int64)
-        inp.queue_constrained_demand = self._ptr(self.qcd, C.c_int64)
-        inp.queue_short_job_penalty = self._ptr(self.qp, C.c_int64)
-        inp.queue_has_limit = self._ptr(self.qhl, C.c_uint8)
-        inp.queue_limit = self._ptr(self.ql, C.c_int64)
-        inp.queue_limiter_tokens = self._ptr(self.qt, C.c_double)
-        inp.queue_limiter_burst = self._ptr(self.qb, C.c_int64)
-        inp.queue_limiter_is_inf = self._ptr(self.qi, C.c_uint8)
+        self._attach(queue_weight=qw, queue_cordoned=qc, queue_allocated_by_pc=qa, queue_demand=qd, queue_constrained_demand=qcd,
+                     queue_short_job_penalty=qp, queue_has_limit=qhl, queue_limit=ql, queue_limiter_tokens=qt,
+                     queue_limiter_burst=qb, queue_limiter_is_inf=qi)
 
-        if queued_order is not None:
-            start = [0]
-            order: List[int] = []
-            for q in self.queues:
-                order += [self.job_pos[jid] for jid in queued_order.get(q.name, [])]
-                start.append(len(order))
-            self.queued_start = a(start, np.uint32)
-            self.queued_order = a(order or [0], np.uint32)
-            inp.queued_start = self._ptr(self.queued_start, C.c_uint32)
-            inp.queued_order = self._ptr(self.queued_order, C.c_uint32)
-        inp._keepalive = self._keep
-        self.input = inp
+    def _queued_order(self, queued_order: Dict[str, List[str]]):
+        """The caller's order of each queue's queued jobs: queues in index order, jobs by position."""
+        start = [0]
+        order: List[int] = []
+        for q in self.queues:
+            order += [self.job_pos[jid] for jid in queued_order.get(q.name, [])]
+            start.append(len(order))
+        self._attach(queued_start=start, queued_order=order or [0])
+
+    # The names the arrays had before they were named after their fields.  Each is a read-only alias of the same
+    # array, so code written against it, in-place writes included, changes what the library reads.
+    FORMER_NAMES = {
+        "qw": "queue_weight", "qc": "queue_cordoned", "qa": "queue_allocated_by_pc", "qd": "queue_demand",
+        "qcd": "queue_constrained_demand", "qp": "queue_short_job_penalty", "qhl": "queue_has_limit", "ql": "queue_limit",
+        "qt": "queue_limiter_tokens", "qb": "queue_limiter_burst", "qi": "queue_limiter_is_inf",
+        "job_qp": "job_queue_priority", "job_st": "job_submit_time", "job_sap": "job_scheduled_at_priority",
+        "job_art": "job_active_run_timestamp", "gang_card": "gang_cardinality", "class_row": "class_static_row",
+        "class_away": "class_away_row", "node_static": "node_static_class", "node_alloc": "node_allocatable",
+    }
+
+
+for _former, _field in RoundInputBuilder.FORMER_NAMES.items():
+    setattr(RoundInputBuilder, _former, property(operator.attrgetter(_field)))
 
 
 class RoundResult:
@@ -751,56 +727,29 @@ class RoundResult:
     def __init__(self, inp: abi.RoundInput, first_pass: Optional[bool] = None):
         J, N, Q = max(inp.num_jobs, 1), max(inp.num_nodes, 1), max(inp.num_queues, 1)
         D, PL, PC = inp.num_resources, inp.num_priorities, inp.num_priority_classes
-        self.job_state = np.zeros(J, np.uint8)
-        self.job_node = np.full(J, abi.NONE, np.uint32)
-        self.job_scheduled_at_priority = np.zeros(J, np.int32)
-        self.job_preempted_at_priority = np.zeros(J, np.int32)
-        self.job_method = np.zeros(J, np.uint8)
-        self.job_reason = np.zeros(J, np.uint8)
-        self.job_seq = np.zeros(J, np.uint32)
-        self.node_alloc = np.zeros((PL, D, N), np.int64)
-        self.queue_allocated = np.zeros((Q, D), np.int64)
-        self.queue_allocated_by_pc = np.zeros((Q, PC, D), np.int64)
-        self.queue_fair_share = np.zeros((Q, 3), np.float64)
-        self.scheduled_resources = np.zeros(D, np.int64)
-        self.evicted_resources = np.zeros(D, np.int64)
-        self.job_excluded_nodes = np.zeros((J, abi.EXCLUDED_KINDS), np.uint32)
-        self.job_seq_first_pass = np.zeros(J, np.uint32)
-        self.job_reason_first_pass = np.zeros(J, np.uint8)
-        o = abi.RoundOutput()
-        o.job_state = self.job_state.ctypes.data_as(abi.u8p)
-        o.job_node = self.job_node.ctypes.data_as(abi.u32p)
-        o.job_scheduled_at_priority = self.job_scheduled_at_priority.ctypes.data_as(abi.i32p)
-        o.job_preempted_at_priority = self.job_preempted_at_priority.ctypes.data_as(abi.i32p)
-        o.job_method = self.job_method.ctypes.data_as(abi.u8p)
-        o.job_reason = self.job_reason.ctypes.data_as(abi.u8p)
-        o.job_seq = self.job_seq.ctypes.data_as(abi.u32p)
-        o.node_alloc = self.node_alloc.ctypes.data_as(abi.i64p)
-        o.queue_allocated = self.queue_allocated.ctypes.data_as(abi.i64p)
-        o.queue_allocated_by_pc = self.queue_allocated_by_pc.ctypes.data_as(abi.i64p)
-        o.queue_fair_share = self.queue_fair_share.ctypes.data_as(abi.f64p)
-        o.scheduled_resources = self.scheduled_resources.ctypes.data_as(abi.i64p)
-        o.evicted_resources = self.evicted_resources.ctypes.data_as(abi.i64p)
-        if inp.collect_excluded_nodes:
-            o.job_excluded_nodes = self.job_excluded_nodes.ctypes.data_as(abi.u32p)
+        shape = {"node_alloc": (PL, D, N), "queue_allocated": (Q, D), "queue_allocated_by_pc": (Q, PC, D), "queue_fair_share": (Q, 3),
+                 "scheduled_resources": D, "evicted_resources": D, "job_excluded_nodes": (J, abi.EXCLUDED_KINDS)}  # the others: [J]
+        arrays = {n: np.zeros(shape.get(n, J), abi.field_dtype(abi.RoundOutput, n)) for n in self.ARRAYS + self.FIRST_PASS_ARRAYS}
+        arrays["job_node"].fill(abi.NONE)
+        vars(self).update(arrays)
         self.first_pass = RoundResult.FIRST_PASS_DEFAULT if first_pass is None else first_pass
-        if self.first_pass:
-            o.job_seq_first_pass = self.job_seq_first_pass.ctypes.data_as(abi.u32p)
-            o.job_reason_first_pass = self.job_reason_first_pass.ctypes.data_as(abi.u8p)
-        self.out = o
+        skip = (() if inp.collect_excluded_nodes else ("job_excluded_nodes",)) + (() if self.first_pass else self.FIRST_PASS_ARRAYS)
+        self.out = abi.RoundOutput()
+        abi.attach(self.out, [], **{n: a for n, a in arrays.items() if n not in skip})  # the arrays live on self
         self.stats = abi.RoundStats()
         self.num_jobs = inp.num_jobs
 
     ARRAYS = ("job_state", "job_node", "job_scheduled_at_priority", "job_preempted_at_priority", "job_method",
               "job_reason", "job_seq", "node_alloc", "queue_allocated", "queue_allocated_by_pc", "queue_fair_share",
               "scheduled_resources", "evicted_resources", "job_excluded_nodes")
+    FIRST_PASS_ARRAYS = ("job_seq_first_pass", "job_reason_first_pass")
     SCALARS = ("num_scheduled_jobs", "num_scheduled_gangs", "num_evicted_jobs", "termination_reason",
                "num_result_scheduled", "num_result_preempted")
 
     def diff(self, other: "RoundResult") -> List[str]:
         """Bit-exact comparison of every output; returns a list of human-readable mismatches."""
         bad = []
-        names = self.ARRAYS + (("job_seq_first_pass", "job_reason_first_pass") if self.first_pass and other.first_pass else ())
+        names = self.ARRAYS + (self.FIRST_PASS_ARRAYS if self.first_pass and other.first_pass else ())
         for name in names:
             x, y = getattr(self, name), getattr(other, name)
             if x.dtype.kind == "f":
@@ -854,7 +803,7 @@ def _eviction_reasons(b: "RoundInputBuilder", res: "RoundResult"):
     total = b.total_resources.astype(np.float64)
     mult = np.array([inp.drf_multipliers[d] for d in range(D)])
     # qctx.GetAllocation() = Allocated + ShortJobPenalty at the start of the round
-    alloc = b.qa.sum(axis=1).astype(np.float64) + b.qp.astype(np.float64)
+    alloc = b.queue_allocated_by_pc.sum(axis=1).astype(np.float64) + b.queue_short_job_penalty.astype(np.float64)
     with np.errstate(divide="ignore", invalid="ignore"):
         frac_d = np.where(total != 0, alloc / np.where(total != 0, total, 1.0), 0.0) * mult
         actual = np.maximum(frac_d.max(axis=1), 0.0) if D else np.zeros(len(b.queues))
@@ -930,7 +879,7 @@ def queue_stats(b: "RoundInputBuilder", res: "RoundResult") -> Dict[str, QueueSt
     running = b.job_node[:J] != abi.NONE
 
     def order_key(j):  # SchedulingOrderCompare (jobdb/comparison.go:49-107)
-        return (0 if running[j] else 1, -pcprio[j], b.job_qp[j], b.job_art[j] if running[j] else 0, b.job_st[j], b.job_id_rank[j])
+        return (0 if running[j] else 1, -pcprio[j], b.job_queue_priority[j], b.job_active_run_timestamp[j] if running[j] else 0, b.job_submit_time[j], b.job_id_rank[j])
 
     evicted = evictable_jobs(b, res)
     total = b.total_resources.astype(np.float64)
@@ -944,7 +893,7 @@ def queue_stats(b: "RoundInputBuilder", res: "RoundResult") -> Dict[str, QueueSt
         gangs: Dict[int, List[int]] = {}
         for j in mine:
             gangs.setdefault(int(seq[j]), []).append(int(j))
-        alloc = b.qa[qi].sum(axis=0) + b.qp[qi]  # qctx.GetAllocation(): Allocated + ShortJobPenalty
+        alloc = b.queue_allocated_by_pc[qi].sum(axis=0) + b.queue_short_job_penalty[qi]  # qctx.GetAllocation(): Allocated + ShortJobPenalty
         for j in np.nonzero((b.job_queue[:J] == qi) & evicted)[0]:
             alloc = alloc - req[j]
         for s in sorted(gangs):
@@ -967,7 +916,7 @@ def queue_stats(b: "RoundInputBuilder", res: "RoundResult") -> Dict[str, QueueSt
                 with np.errstate(divide="ignore", invalid="ignore"):
                     frac = np.where(total != 0, alloc / np.where(total != 0, total, 1.0), 0.0) * mult
                 cost = max(float(frac.max()), 0.0) if f.D else 0.0
-                st.last_gang_scheduled_queue_cost = cost / float(b.qw[qi])
+                st.last_gang_scheduled_queue_cost = cost / float(b.queue_weight[qi])
         out[q.name] = st
     return out
 
@@ -1096,9 +1045,9 @@ def last_probe_row(b: "RoundInputBuilder", cls: int) -> Optional[int]:
     on, else the home row when home scheduling is on; None when no probe runs."""
     if not b.cfg.disable_away_scheduling:
         for k in reversed(range(abi.MAX_AWAY)):
-            if int(b.class_away[cls, k]) != abi.NONE:
-                return int(b.class_away[cls, k])
-    return None if b.cfg.disable_home_scheduling else int(b.class_row[cls])
+            if int(b.class_away_row[cls, k]) != abi.NONE:
+                return int(b.class_away_row[cls, k])
+    return None if b.cfg.disable_home_scheduling else int(b.class_static_row[cls])
 
 
 def excluded_nodes_by_reason(b: "RoundInputBuilder", cls: int, records) -> Dict[str, int]:

@@ -10,7 +10,6 @@ TestResources index resolutions (:108-112), factory order memory, cpu, gpu (:124
 """
 from __future__ import annotations
 
-import ctypes as C
 from dataclasses import dataclass, field
 from typing import Dict, List, Optional, Sequence, Tuple
 
@@ -93,16 +92,6 @@ class RawRound:
     _keep: list = field(default_factory=list)
 
     def to_input(self) -> abi.RoundInput:
-        self._keep = []
-
-        def arr(a, dt):
-            a = np.ascontiguousarray(a, dtype=dt)
-            self._keep.append(a)
-            return a
-
-        def ptr(a, ct):
-            return a.ctypes.data_as(C.POINTER(ct))
-
         inp = abi.RoundInput()
         inp.abi_version = abi.ABI_VERSION
         D = self.node_total.shape[0]
@@ -143,53 +132,17 @@ class RawRound:
         inp.global_limiter_burst = self.global_burst
         inp.global_limiter_tokens = float(self.global_burst) if self.global_tokens is None else self.global_tokens
         inp.num_nodes, inp.num_node_types, inp.num_static_classes = N, self.num_node_types, self.num_static_classes
-        node_index = self.node_index if self.node_index is not None else np.arange(N)
-        node_id_rank = self.node_id_rank if self.node_id_rank is not None else np.arange(N)
-        inp.node_index = ptr(arr(node_index, np.uint64), C.c_uint64)
-        inp.node_id_rank = ptr(arr(node_id_rank, np.uint32), C.c_uint32)
-        inp.node_type = ptr(arr(self.node_type, np.uint32), C.c_uint32)
-        inp.node_static_class = ptr(arr(self.node_static_class, np.uint32), C.c_uint32)
-        inp.node_flags = ptr(arr(self.node_flags if self.node_flags is not None else np.zeros(N), np.uint8), C.c_uint8)
-        inp.node_total = ptr(arr(self.node_total, np.int64), C.c_int64)
-        inp.node_allocatable = ptr(arr(self.node_allocatable, np.int64), C.c_int64)
         inp.num_classes = Cn
         inp.num_static_rows = self.static_match.shape[0]
-        inp.class_request = ptr(arr(self.class_request, np.int64), C.c_int64)
-        inp.class_pc = ptr(arr(self.class_pc, np.uint32), C.c_uint32)
-        inp.class_static_row = ptr(arr(self.class_static_row, np.uint32), C.c_uint32)
-        away = self.class_away_row if self.class_away_row is not None else np.full((Cn, abi.MAX_AWAY), abi.NONE)
-        inp.class_away_row = ptr(arr(away, np.uint32), C.c_uint32)
-        inp.class_key_valid = ptr(arr(np.ones(Cn), np.uint8), C.c_uint8)
-        inp.static_match = ptr(arr(self.static_match, np.uint32), C.c_uint32)
-        inp.type_match = ptr(arr(self.type_match, np.uint32), C.c_uint32)
         inp.num_jobs = J
-        gang = self.job_gang if self.job_gang is not None else np.full(J, abi.NONE)
-        gcard = self.gang_cardinality if self.gang_cardinality is not None else np.zeros(1)
         inp.num_gangs = 0 if self.gang_cardinality is None else len(self.gang_cardinality)
-        job_node = self.job_node if self.job_node is not None else np.full(J, abi.NONE)
-        sap = self.job_scheduled_at_priority if self.job_scheduled_at_priority is not None else np.full(J, abi.NO_PRIORITY)
-        art = self.job_active_run_timestamp if self.job_active_run_timestamp is not None else np.zeros(J)
-        qprio = self.job_queue_priority if self.job_queue_priority is not None else np.full(J, 1000)
-        inp.job_class = ptr(arr(self.job_class, np.uint32), C.c_uint32)
-        inp.job_queue = ptr(arr(self.job_queue, np.uint32), C.c_uint32)
-        inp.job_queue_priority = ptr(arr(qprio, np.uint32), C.c_uint32)
-        inp.job_submit_time = ptr(arr(self.job_submit_time, np.int64), C.c_int64)
-        inp.job_id_rank = ptr(arr(np.arange(J), np.uint32), C.c_uint32)
-        inp.job_gang = ptr(arr(gang, np.uint32), C.c_uint32)
-        inp.job_node = ptr(arr(job_node, np.uint32), C.c_uint32)
-        inp.job_scheduled_at_priority = ptr(arr(sap, np.int32), C.c_int32)
-        inp.job_active_run_timestamp = ptr(arr(art, np.int64), C.c_int64)
-        inp.gang_cardinality = ptr(arr(gcard, np.uint32), C.c_uint32)
         inp.num_queues = Q
-        inp.queue_weight = ptr(arr(self.queue_weight, np.float64), C.c_double)
-        inp.queue_cordoned = ptr(arr(np.zeros(Q), np.uint8), C.c_uint8)
+        job_node = self.job_node if self.job_node is not None else np.full(J, abi.NONE)
         # queue accounting derived from the job arrays (calculateJobSchedulingInfo, scheduling_algo.go:522-632)
-        job_node_a = np.asarray(job_node)
         jq = np.asarray(self.job_queue).astype(np.int64)
-        job_node_a = job_node_a.astype(np.int64)
         req = np.asarray(self.class_request)[np.asarray(self.job_class).astype(np.int64)]  # [J][D]
         has_q = jq != abi.NONE
-        running = (job_node_a != abi.NONE) & has_q
+        running = (np.asarray(job_node).astype(np.int64) != abi.NONE) & has_q
         demand = np.zeros((Q, D), np.int64)
         np.add.at(demand, jq[has_q], req[has_q])
         if self.queue_allocated_by_pc is not None:
@@ -198,20 +151,31 @@ class RawRound:
             alloc_pc = np.zeros((Q, PCn, D), np.int64)
             jpc = np.asarray(self.class_pc)[np.asarray(self.job_class).astype(np.int64)].astype(np.int64)
             np.add.at(alloc_pc, (jq[running], jpc[running]), req[running])
-        inp.queue_allocated_by_pc = ptr(arr(alloc_pc, np.int64), C.c_int64)
-        inp.queue_demand = ptr(arr(demand, np.int64), C.c_int64)
-        inp.queue_constrained_demand = ptr(arr(demand, np.int64), C.c_int64)
-        inp.queue_short_job_penalty = ptr(arr(np.zeros((Q, D)), np.int64), C.c_int64)
-        if self.queue_limit is not None:
-            inp.queue_has_limit = ptr(arr(np.ones((Q, PCn)), np.uint8), C.c_uint8)
-            inp.queue_limit = ptr(arr(self.queue_limit, np.int64), C.c_int64)
-        else:
-            inp.queue_has_limit = ptr(arr(np.zeros((Q, PCn)), np.uint8), C.c_uint8)
-            inp.queue_limit = ptr(arr(np.zeros((Q, PCn, D)), np.int64), C.c_int64)
-        inp.queue_limiter_tokens = ptr(arr(np.full(Q, float(2**62)), np.float64), C.c_double)
-        inp.queue_limiter_burst = ptr(arr(np.full(Q, 2**62), np.int64), C.c_int64)
-        inp.queue_limiter_is_inf = ptr(arr(np.ones(Q), np.uint8), C.c_uint8)
-        inp._keepalive = self._keep  # the struct only holds raw pointers into these arrays
+        self._keep = []  # the struct only holds raw pointers into these arrays
+        abi.attach(
+            inp, self._keep,
+            node_index=self.node_index if self.node_index is not None else np.arange(N),
+            node_id_rank=self.node_id_rank if self.node_id_rank is not None else np.arange(N),
+            node_type=self.node_type, node_static_class=self.node_static_class,
+            node_flags=self.node_flags if self.node_flags is not None else np.zeros(N),
+            node_total=self.node_total, node_allocatable=self.node_allocatable,
+            class_request=self.class_request, class_pc=self.class_pc, class_static_row=self.class_static_row,
+            class_away_row=self.class_away_row if self.class_away_row is not None else np.full((Cn, abi.MAX_AWAY), abi.NONE),
+            class_key_valid=np.ones(Cn), static_match=self.static_match, type_match=self.type_match,
+            job_class=self.job_class, job_queue=self.job_queue,
+            job_queue_priority=self.job_queue_priority if self.job_queue_priority is not None else np.full(J, 1000),
+            job_submit_time=self.job_submit_time, job_id_rank=np.arange(J),
+            job_gang=self.job_gang if self.job_gang is not None else np.full(J, abi.NONE), job_node=job_node,
+            job_scheduled_at_priority=(self.job_scheduled_at_priority if self.job_scheduled_at_priority is not None
+                                       else np.full(J, abi.NO_PRIORITY)),
+            job_active_run_timestamp=self.job_active_run_timestamp if self.job_active_run_timestamp is not None else np.zeros(J),
+            gang_cardinality=self.gang_cardinality if self.gang_cardinality is not None else np.zeros(1),
+            queue_weight=self.queue_weight, queue_cordoned=np.zeros(Q), queue_allocated_by_pc=alloc_pc,
+            queue_demand=demand, queue_constrained_demand=demand, queue_short_job_penalty=np.zeros((Q, D)),
+            queue_has_limit=np.ones((Q, PCn)) if self.queue_limit is not None else np.zeros((Q, PCn)),
+            queue_limit=self.queue_limit if self.queue_limit is not None else np.zeros((Q, PCn, D)),
+            queue_limiter_tokens=np.full(Q, float(2**62)), queue_limiter_burst=np.full(Q, 2**62), queue_limiter_is_inf=np.ones(Q))
+        inp._keepalive = self._keep
         self.input = inp
         return inp
 

@@ -169,20 +169,20 @@ def _records(b, cls, odb, N, D, nodes_of_type, sw, tw):
         pc = inp.priority_classes[int(b.class_pc[cls])]
         sched_at = pc.priority
         for k in range(abi.MAX_AWAY):
-            if int(b.class_away[cls, k]) == row and not b.cfg.disable_away_scheduling:
+            if int(b.class_away_row[cls, k]) == row and not b.cfg.disable_away_scheduling:
                 sched_at = pc.away_priority[k]
         for t in range(inp.num_node_types):
             if not (int(b.type_match[row, t >> 5]) >> (t & 31)) & 1 and nodes_of_type[t]:
                 recs[(abi.EXCL_NODE_TYPE, t, 0)] = int(nodes_of_type[t])
         ireq = [int(req[inp.indexed_resource[i]]) for i in range(inp.num_indexed)]
         for n in odb.iterate(row, sched_at, ireq):
-            s = int(b.node_static[n])
+            s = int(b.node_static_class[n])
             if not (int(b.static_match[row, s >> 5]) >> (s & 31)) & 1:
                 key = (abi.EXCL_STATIC, s, 0)
             else:
                 dt = [d for d in range(D) if req[d] > b.node_total[d, n]]
-                da = [d for d in range(D) if req[d] > b.node_alloc[d, n]]
-                key = (abi.EXCL_STATIC_TOTAL, dt[0], int(b.node_total[dt[0], n])) if dt else (abi.EXCL_RESOURCES, da[0], int(b.node_alloc[da[0], n]))
+                da = [d for d in range(D) if req[d] > b.node_allocatable[d, n]]
+                key = (abi.EXCL_STATIC_TOTAL, dt[0], int(b.node_total[dt[0], n])) if dt else (abi.EXCL_RESOURCES, da[0], int(b.node_allocatable[da[0], n]))
             recs[key] = recs.get(key, 0) + 1
     rest = N - sum(recs.values())
     if rest > 0:

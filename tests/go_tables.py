@@ -528,5 +528,5 @@ def run_pqs_case(case: dict, run_round: Callable, check_expected: bool = True, o
         if not math.isinf(cfg.maximum_per_queue_scheduling_rate):
             for qn in pf_by_queue:
                 used = sum(1 for j in queued if j.queue == qn and states[j.id] == abi.JOB_SCHEDULED)
-                cur = float(b.qt[b.queue_index[qn]]) - used
-                tokens_queue[qn] = min(float(b.qb[b.queue_index[qn]]), cur + cfg.maximum_per_queue_scheduling_rate * 1.0)
+                cur = float(b.queue_limiter_tokens[b.queue_index[qn]]) - used
+                tokens_queue[qn] = min(float(b.queue_limiter_burst[b.queue_index[qn]]), cur + cfg.maximum_per_queue_scheduling_rate * 1.0)

@@ -78,7 +78,7 @@ def test_calculate_fair_shares(name):
     total = f.from_node(tc["availableResources"])
     b = RoundInputBuilder(cfg, [fx.Fixtures().cpu32()], [], queues, total_resources=total)
     for qn, w in weights.items():  # the test passes weights directly (not 1/priorityFactor)
-        b.qw[b.queue_index[qn]] = w
+        b.queue_weight[b.queue_index[qn]] = w
     res = oracle_lib.round_schedule(b.input)
     for qn in weights:
         qi = b.queue_index[qn]
@@ -292,7 +292,7 @@ def test_per_queue_limits(name, pc_fraction, queue_fraction, want):
     f = cfg.factory()
     total = f.from_node({"cpu": "1000", "memory": "1000Gi"})
     b = RoundInputBuilder(cfg, [], [], [q], total_resources=total)
-    got = b.ql[0, 0]
+    got = b.queue_limit[0, 0]
     if want is None:  # rlFactory.MakeAllMax()
         assert (got == 2**63 - 1).all()
     else:
@@ -358,7 +358,7 @@ def test_queue_stats_from_the_first_pass_view(seed):
         if int(res.stats.evicted_pass2) == 0 and st.gangs_scheduled:
             # nothing moved after the first pass: the replay's last allocation (incl. the short-job penalty, zero here)
             # is the queue's final allocation
-            assert (st.last_gang_scheduled_queue_resources == res.queue_allocated[qi] + b.qp[qi]).all()
+            assert (st.last_gang_scheduled_queue_resources == res.queue_allocated[qi] + b.queue_short_job_penalty[qi]).all()
     assert 0 in positions  # some queue was looked at in the very first iteration
 
 

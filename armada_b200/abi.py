@@ -252,6 +252,8 @@ def declare_prototypes(lib: C.CDLL) -> None:
     lib.armada_nodedb_explain.restype = C.c_int32
     lib.armada_nodedb_select_nodes.argtypes = [vp, C.c_uint32, u32p, u32p]
     lib.armada_nodedb_select_nodes.restype = C.c_int32
+    lib.armada_nodedb_add_classes.argtypes = [vp, C.c_uint32, i64p, u32p, u32p, u32p, u8p, C.c_uint32, u32p, u32p, u32p]
+    lib.armada_nodedb_add_classes.restype = C.c_int32
     lib.armada_nodedb_destroy.argtypes = [vp]
     lib.armada_nodedb_destroy.restype = C.c_int32
     lib.armada_strerror.argtypes = [C.c_int32]
@@ -289,6 +291,7 @@ PRODUCT_SYMBOLS = [
     "armada_nodedb_schedule_many",
     "armada_nodedb_explain",
     "armada_nodedb_select_nodes",
+    "armada_nodedb_add_classes",
     "armada_nodedb_destroy",
     "armada_strerror",
     "armada_last_error",

@@ -282,6 +282,16 @@ def multiply_resource(res: int, m: float) -> int:
     return int(v)
 
 
+class UnresolvedLabels(ValueError):
+    """RoundInputBuilder.add_jobs: a new row looks at a node label the builder's static classes do not resolve."""
+
+
+def scheduling_key(j: JobSpec, req: np.ndarray):
+    """A job's class: the fields of its SchedulingKey (node selector, affinity, tolerations, requests, priority
+    class; internaltypes/podutils.go:49-68), `req` being its requests in factory units."""
+    return (tuple(sorted(j.tolerations, key=repr)), tuple(sorted(j.node_selector.items())), j.affinity, tuple(int(x) for x in req), j.priority_class)
+
+
 class RoundInputBuilder:
     """Flattens (config, nodes, jobs, queues) into an ArmadaRoundInput.  Every array the input points into is the
     builder's attribute of the field's name and lives as long as the builder."""
@@ -399,24 +409,34 @@ class RoundInputBuilder:
     def _job_classes(self) -> List[Tuple[Tuple[Toleration, ...], Dict[str, str], object, List[Tuple[Toleration, ...]]]]:
         """Job classes with their home and away rows, and each job's class.  Returns per class its tolerations,
         selector, affinity and per away node type the tolerations it adds, from which the uniformity rows are made."""
+        self._classes: Dict[object, int] = {}
+        self._class_req: List[np.ndarray] = []
+        self._class_pc: List[int] = []
+        self._class_row: List[int] = []
+        self._class_away: List[List[int]] = []
+        self._class_meta: List[Tuple[Tuple[Toleration, ...], Dict[str, str], object, List[Tuple[Toleration, ...]]]] = []
+        self.class_jobs: List[JobSpec] = []  # the first job of each class (none for the placeholder class)
+        job_class = self._register(self.jobs)
+        if not self._class_req:  # keep arrays non-empty for the C side (no jobs: no uniformity rows follow this row); no job has this class
+            self._class_req, self._class_pc, self._class_row = [np.zeros(self.factory.D, np.int64)], [0], [self._row((), {}, None)]
+            self._class_away = [[abi.NONE] * abi.MAX_AWAY]
+        self._attach_classes()
+        self._attach(job_class=job_class if self.jobs else [0])
+        return self._class_meta
+
+    def _register(self, jobs: Sequence[JobSpec]) -> np.ndarray:
+        """The class of each job, registering the classes (and their rows) not seen before."""
         cfg, f = self.cfg, self.factory
-        classes: Dict[object, int] = {}
-        class_req: List[np.ndarray] = []
-        class_pc: List[int] = []
-        class_row: List[int] = []
-        class_away: List[List[int]] = []
-        class_meta: List[Tuple[Tuple[Toleration, ...], Dict[str, str], object, List[Tuple[Toleration, ...]]]] = []
-        job_class = np.zeros(len(self.jobs), dtype=np.uint32)
-        for ji, j in enumerate(self.jobs):
+        job_class = np.zeros(len(jobs), dtype=np.uint32)
+        for ji, j in enumerate(jobs):
             req = f.from_job(j.requests)
-            key = (tuple(sorted(j.tolerations, key=repr)), tuple(sorted(j.node_selector.items())), j.affinity,
-                   tuple(int(x) for x in req), j.priority_class)
-            if key not in classes:
-                classes[key] = len(class_req)
-                class_req.append(req)
+            key = scheduling_key(j, req)
+            if key not in self._classes:
+                self._classes[key] = len(self._class_req)
+                self._class_req.append(req)
                 pc = cfg.priority_classes[j.priority_class]
-                class_pc.append(self.pc_index[j.priority_class])
-                class_row.append(self._row(j.tolerations, j.node_selector, j.affinity))
+                self._class_pc.append(self.pc_index[j.priority_class])
+                self._class_row.append(self._row(j.tolerations, j.node_selector, j.affinity))
                 aw = [abi.NONE] * abi.MAX_AWAY
                 extras: List[Tuple[Toleration, ...]] = []
                 for k in range(len(pc.away_node_types)):
@@ -424,15 +444,56 @@ class RoundInputBuilder:
                     extras.append(extra)
                     if extra:
                         aw[k] = self._row(tuple(j.tolerations) + extra, j.node_selector, j.affinity)
-                class_away.append(aw)
-                class_meta.append((tuple(j.tolerations), dict(j.node_selector), j.affinity, extras))
-            job_class[ji] = classes[key]
-        if not class_req:  # keep arrays non-empty for the C side (no jobs: no uniformity rows follow this row)
-            class_req, class_pc, class_row, class_away = [np.zeros(f.D, np.int64)], [0], [self._row((), {}, None)], [[abi.NONE] * abi.MAX_AWAY]
-        self.input.num_classes = len(class_req)
-        self._attach(class_request=np.stack(class_req), class_pc=class_pc, class_static_row=class_row, class_away_row=class_away,
-                     class_key_valid=np.ones(len(class_req)), job_class=job_class if self.jobs else [0])
-        return class_meta
+                self._class_away.append(aw)
+                self._class_meta.append((tuple(j.tolerations), dict(j.node_selector), j.affinity, extras))
+                self.class_jobs.append(j)
+            job_class[ji] = self._classes[key]
+        return job_class
+
+    def _attach_classes(self):
+        self.input.num_classes = len(self._class_req)
+        self._attach(class_request=np.stack(self._class_req), class_pc=self._class_pc, class_static_row=self._class_row,
+                     class_away_row=self._class_away, class_key_valid=np.ones(len(self._class_req)))
+
+    def add_jobs(self, jobs: Sequence[JobSpec]) -> Tuple[np.ndarray, range, range]:
+        """Register the classes of `jobs` (scheduling keys) against the builder's fixed node static classes and node
+        types: the class arrays, row table and bitmaps grow, the nodes stay.  Returns each job's class, the new
+        classes and the new rows (what armada_nodedb_add_classes appends to a NodeDb made from this builder's
+        input).  Classes and rows get the ids a builder made with all the jobs at once gives them, as long as no
+        placeholder class was made.  Raises UnresolvedLabels, the builder unchanged, when a new row looks at a node
+        label the static classes do not tell apart (only labels the rows so far look at do): such jobs need a
+        builder made with them.  Gang node uniformity is not registered (the dry-run NodeDb has none)."""
+        c0, r0 = len(self._class_req), len(self.row_specs)
+        job_class = self._register(jobs)
+        for r in range(r0, len(self.row_specs)):
+            _, selector, affinity = self.row_specs[r]
+            keys = {k for k, _ in selector} | {e.key for term in (affinity or ()) for e in term}
+            unresolved = sorted(k for k in keys if k in self.node_label_keys and k not in self.static_label_keys)
+            if unresolved:
+                self.rollback(c0, r0)
+                raise UnresolvedLabels(f"the static classes do not tell nodes apart by label(s) {unresolved}")
+        if len(self._class_req) > c0:
+            self._attach_classes()
+        if len(self.row_specs) > r0:
+            sm, tm = self._match_rows(r0, len(self.row_specs))
+            self.input.num_static_rows = len(self.row_specs)
+            self._attach(static_match=np.concatenate([self.static_match, sm]), type_match=np.concatenate([self.type_match, tm]))
+        return job_class, range(c0, len(self._class_req)), range(r0, len(self.row_specs))
+
+    def rollback(self, num_classes: int, num_rows: int) -> None:
+        """Forget the classes and rows from `num_classes` / `num_rows` on: what add_jobs registered since the
+        builder had that many (when the db they were meant for refused them)."""
+        for key in [k for k, c in self._classes.items() if c >= num_classes]:
+            del self._classes[key]
+        for seq in (self._class_req, self._class_pc, self._class_row, self._class_away, self._class_meta):
+            del seq[num_classes:]
+        del self.class_jobs[len(self._classes):]  # (the placeholder class has no key and no job)
+        for key in [k for k, r in self._rows.items() if r >= num_rows]:
+            del self._rows[key]
+        del self.row_specs[num_rows:]
+        self._attach_classes()
+        self.input.num_static_rows = num_rows
+        self._attach(static_match=self.static_match[:num_rows], type_match=self.type_match[:num_rows])
 
     def _uniformity_rows(self, class_meta) -> np.ndarray:
         """Gang node uniformity (gang_scheduler.go:154-223): value slots per label, rows per (class, slot).  Adds
@@ -518,6 +579,7 @@ class RoundInputBuilder:
             node_flags[i] = (abi.NODE_UNSCHEDULABLE if n.unschedulable else 0) | (abi.NODE_OVERALLOCATED if n.over_allocated else 0)
         inp.num_static_classes, inp.num_node_types = max(1, len(static_specs)), max(1, len(type_specs))
         self.static_specs, self.type_specs = static_specs, type_specs
+        self.static_label_keys, self.node_label_keys = rel_keys, {k for n in self.nodes for k in self._node_labels(n)}
         self.type_keys = list(types.keys())
         self._attach(node_index=[n.index for n in self.nodes] or [0], node_id_rank=id_rank if N else [0],
                      node_type=node_type if N else [0], node_static_class=node_static if N else [0],
@@ -526,12 +588,16 @@ class RoundInputBuilder:
 
     def _match(self):
         """Per row, the static classes (static_match) and node types (type_match) its requirements admit."""
+        self.input.num_static_rows = len(self.row_specs)
+        static_match, type_match = self._match_rows(0, len(self.row_specs))
+        self._attach(static_match=static_match, type_match=type_match)
+
+    def _match_rows(self, r0: int, r1: int) -> Tuple[np.ndarray, np.ndarray]:
+        """static_match and type_match of rows [r0, r1)."""
         S, T = self.input.num_static_classes, self.input.num_node_types
-        nrows = len(self.row_specs)
-        self.input.num_static_rows = nrows
-        static_match = np.zeros((nrows, (S + 31) // 32), dtype=np.uint32)
-        type_match = np.zeros((nrows, (T + 31) // 32), dtype=np.uint32)
-        for r, (tolerations, selector, affinity) in enumerate(self.row_specs):
+        static_match = np.zeros((r1 - r0, (S + 31) // 32), dtype=np.uint32)
+        type_match = np.zeros((r1 - r0, (T + 31) // 32), dtype=np.uint32)
+        for r, (tolerations, selector, affinity) in enumerate(self.row_specs[r0:r1]):
             for s, (taints, labels) in enumerate(self.static_specs):
                 ok = find_untolerated(taints, tolerations) is None  # NodeTolerationRequirementsMet
                 ok = ok and all(labels.get(k) == v for k, v in selector)  # NodeSelectorRequirementsMet(node, nil)
@@ -552,7 +618,7 @@ class RoundInputBuilder:
                             break
                 if ok:
                     type_match[r, t >> 5] |= np.uint32(1 << (t & 31))
-        self._attach(static_match=static_match, type_match=type_match)
+        return static_match, type_match
 
     def _jobs(self, class_uniformity_row: np.ndarray):
         """Per-job arrays, gangs and the gangs' uniformity labels."""

@@ -169,6 +169,35 @@ class DeviceNodeDb:
             raise abi.ArmadaError(st, f"{self.lib.armada_strerror(st).decode()}: {self.lib.armada_last_error().decode()}")
         return node[: len(list(classes))]
 
+    def add_classes(self, class_request, class_pc, class_static_row, class_away_row, static_match, type_match) -> int:
+        """armada_nodedb_add_classes: append job classes ([n][D] requests, [n] priority-class indices, [n] home
+        rows, [n][MAX_AWAY] away rows) and bitmap rows ([m][sw] static_match, [m][tw] type_match, against the
+        db's static classes and node types).  Returns the id of the first new class; raises ArmadaError and
+        leaves the db as it was when the library refuses them."""
+        import numpy as np
+        inp = self._input
+        pc = np.ascontiguousarray(class_pc, np.uint32).reshape(-1)
+        n = len(pc)
+        # the library reads these widths from raw pointers: a wrong shape is refused here
+        shapes = {"class_request": (n, inp.num_resources), "class_static_row": (n,), "class_away_row": (n, abi.MAX_AWAY)}
+        req = np.ascontiguousarray(class_request, np.int64)
+        row = np.ascontiguousarray(class_static_row, np.uint32)
+        away = np.ascontiguousarray(class_away_row, np.uint32)
+        sm = np.ascontiguousarray(static_match, np.uint32)
+        tm = np.ascontiguousarray(type_match, np.uint32)
+        shapes.update(static_match=(len(sm), (inp.num_static_classes + 31) // 32), type_match=(len(sm), (inp.num_node_types + 31) // 32))
+        for name, a in (("class_request", req), ("class_static_row", row), ("class_away_row", away), ("static_match", sm), ("type_match", tm)):
+            if a.shape != shapes[name]:
+                raise ValueError(f"{name} has shape {a.shape}, the db needs {shapes[name]}")
+        valid = np.ones(max(n, 1), np.uint8)
+        first = C.c_uint32(0)
+        ptr = lambda a, t: a.ctypes.data_as(t) if a.size else None  # noqa: E731
+        st = self.lib.armada_nodedb_add_classes(self.h, n, ptr(req.reshape(-1), abi.i64p), ptr(pc, abi.u32p), ptr(row, abi.u32p), ptr(away.reshape(-1), abi.u32p),
+                                                valid.ctypes.data_as(abi.u8p), len(sm), ptr(sm, abi.u32p), ptr(tm, abi.u32p), C.byref(first))
+        if st != abi.OK:
+            raise abi.ArmadaError(st, f"{self.lib.armada_strerror(st).decode()}: {self.lib.armada_last_error().decode()}")
+        return first.value
+
     def close(self):
         if self.h:
             self.lib.armada_nodedb_destroy(self.h)
@@ -179,3 +208,9 @@ class DeviceNodeDb:
 
     def __exit__(self, *exc):
         self.close()
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass

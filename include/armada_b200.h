@@ -412,6 +412,17 @@ int32_t armada_nodedb_explain(ArmadaNodeDb* db, uint32_t num_gangs, const uint32
  * cluster — what SubmitChecker does for a single job (submitcheck.go:353-371): node[i] = the node job i
  * (a job-class index of `in`) would be bound to, ARMADA_NONE = it fits nowhere. */
 int32_t armada_nodedb_select_nodes(ArmadaNodeDb* db, uint32_t num_jobs, const uint32_t* job_class, uint32_t* node);
+/* Append job classes (scheduling keys) to a dry-run NodeDb without touching its nodes.  The new classes get
+ * ids db_classes .. db_classes + num_classes - 1 (*first_id).  Their static rows index the db's bitmap
+ * rows; rows [db_rows, db_rows + num_rows) are appended from static_match / type_match (same layout
+ * as ArmadaRoundInput, against the static classes and node types the db was created with).  The new
+ * classes are validated as armada_nodedb_create validates its classes.  On any error nothing is changed.
+ * What a SubmitChecker does with one NodeDb per executor across Check calls (submitcheck.go:132-267). */
+int32_t armada_nodedb_add_classes(ArmadaNodeDb* db, uint32_t num_classes, const int64_t* class_request,
+                                  const uint32_t* class_pc, const uint32_t* class_static_row,
+                                  const uint32_t* class_away_row, const uint8_t* class_key_valid,
+                                  uint32_t num_rows, const uint32_t* static_match, const uint32_t* type_match,
+                                  uint32_t* first_id);
 int32_t armada_nodedb_destroy(ArmadaNodeDb* db);
 
 const char* armada_strerror(int32_t status);

@@ -46,6 +46,19 @@ enum StatSlot {
   STAT_COUNT = 50,
 };
 
+// Slots of DevPtrs::s_counts: the round's sctx counts, carried from kernel to kernel (k_reset sets them; the schedule
+// pass loads them in its prologue and stores them back in its epilogue).
+enum CountSlot {
+  CNT_SCHED_JOBS = 0,     // numScheduledJobs
+  CNT_SCHED_GANGS = 1,    // numScheduledGangs
+  CNT_EVICTED_JOBS = 2,   // numEvictedJobs
+  CNT_TERMINATION = 3,    // termination reason of the first pass
+  CNT_GLOBAL_TOKENS = 4,  // global rate-limiter tokens (double bits)
+  CNT_ERROR = 5,          // error code of the passes (0 = none; an error of the first pass survives the second)
+  CNT_COUNT = 8,
+};
+#define ARMADA_DEV_E_DEADLINE 100  // CNT_ERROR: a pass ran out of its time budget (PassArgs::budget_ns)
+
 struct DevCfg {  // small POD, lives in global memory, hot parts copied to smem
   int32_t D, R, PL, PC, Q, C, T, S, rows;
   uint32_t N, J, G;
@@ -213,8 +226,7 @@ struct DevPtrs {
   double* q_tokens;                // [Q]
   int64_t* s_scheduled;            // [D]
   int64_t* s_evicted;              // [D]
-  int64_t* s_counts;               // [8]: 0 numScheduledJobs 1 numScheduledGangs 2 numEvictedJobs
-                                   //      3 termination(pass1) 4 global tokens (double bits)
+  int64_t* s_counts;               // [CNT_COUNT] (CountSlot)
   uint32_t* dbg_host;              // [64] host-mapped: written by the device watchdog before it traps
   unsigned long long* stats;       // [STAT_COUNT] counters of the round's schedule passes (StatSlot)
 };

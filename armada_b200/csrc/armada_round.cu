@@ -177,8 +177,8 @@ __global__ void k_queue_init(DevCfg c, DevPtrs P) {
     weight_sum += P.queue_weight[q];
   }
   for (int d = 0; d < D; ++d) P.s_scheduled[d] = P.s_evicted[d] = 0;
-  for (int k = 0; k < 8; ++k) P.s_counts[k] = 0;
-  P.s_counts[4] = __double_as_longlong(c.global_tokens);
+  for (int k = 0; k < CNT_COUNT; ++k) P.s_counts[k] = 0;
+  P.s_counts[CNT_GLOBAL_TOKENS] = __double_as_longlong(c.global_tokens);
   bool total_all_zero = true;
   for (int d = 0; d < D; ++d)
     if (c.total_resources[d] != 0) total_all_zero = false;
@@ -346,8 +346,8 @@ __global__ void k_evict_account(DevCfg c, DevPtrs P, int pass) {
     if (sched) atomic_add_i64(&P.s_scheduled[d], -r);
     else atomic_add_i64(&P.s_evicted[d], r);
   }
-  if (sched) atomic_add_i64(&P.s_counts[0], -1);
-  else atomic_add_i64(&P.s_counts[2], 1);
+  if (sched) atomic_add_i64(&P.s_counts[CNT_SCHED_JOBS], -1);
+  else atomic_add_i64(&P.s_counts[CNT_EVICTED_JOBS], 1);
   // jctx for re-scheduling (eviction.go:241-256)
   P.jc_evicted[j] = 1;
   P.assigned_node[j] = P.bound_node[j];

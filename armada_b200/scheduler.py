@@ -15,6 +15,11 @@ from . import abi
 from .model import RoundResult, excluded_nodes_by_reason
 
 
+def _check(lib, status: int) -> None:
+    if status != abi.OK:
+        raise abi.ArmadaError(status, f"{lib.armada_strerror(status).decode()}: {lib.armada_last_error().decode()}")
+
+
 class DeviceRound:
     """Owns one `ArmadaRound*` (device context).  upload → run → download, like
     populateNodeDb → Schedule → result read-back in scheduling_algo.go:740-840."""
@@ -24,31 +29,24 @@ class DeviceRound:
         # emulator); the product always loads the CUDA library and fails loudly without it.
         self.lib = lib if lib is not None else abi.load_product()
         self.h = C.c_void_p()
-        self._check(self.lib.armada_round_create(device, C.byref(self.h)))
+        _check(self.lib, self.lib.armada_round_create(device, C.byref(self.h)))
         self._input: Optional[abi.RoundInput] = None
 
-    def _check(self, status: int):
-        if status != abi.OK:
-            raise abi.ArmadaError(status, f"{self.lib.armada_strerror(status).decode()}: {self.lib.armada_last_error().decode()}")
-
     def upload(self, inp: abi.RoundInput) -> None:
-        self._check(self.lib.armada_round_upload(self.h, C.byref(inp)))
+        _check(self.lib, self.lib.armada_round_upload(self.h, C.byref(inp)))
         self._input = inp
 
     def run(self, budget_ns: int = 0) -> abi.RoundStats:
         """`budget_ns` > 0: the cycle's maxSchedulingDuration (scheduling_algo.go:115-118); raises
         ArmadaError(E_DEADLINE) when it runs out — nothing of the round is committed."""
         stats = abi.RoundStats()
-        if budget_ns:
-            self._check(self.lib.armada_round_run_deadline(self.h, C.byref(stats), int(budget_ns)))
-        else:
-            self._check(self.lib.armada_round_run(self.h, C.byref(stats)))
+        _check(self.lib, self.lib.armada_round_run_deadline(self.h, C.byref(stats), int(budget_ns)))
         return stats
 
     def download(self, res: Optional[RoundResult] = None) -> RoundResult:
         if res is None:
             res = RoundResult(self._input)
-        self._check(self.lib.armada_round_download(self.h, C.byref(res.out)))
+        _check(self.lib, self.lib.armada_round_download(self.h, C.byref(res.out)))
         return res
 
     def schedule(self, inp: abi.RoundInput, res: Optional[RoundResult] = None) -> RoundResult:
@@ -56,7 +54,7 @@ class DeviceRound:
         if res is None:
             res = RoundResult(inp)
         self._input = inp
-        self._check(self.lib.armada_round_schedule(self.h, C.byref(inp), C.byref(res.out), C.byref(res.stats)))
+        _check(self.lib, self.lib.armada_round_schedule(self.h, C.byref(inp), C.byref(res.out), C.byref(res.stats)))
         return res
 
     def close(self):
@@ -93,6 +91,18 @@ def round_schedule(inp: abi.RoundInput, device: int = 0) -> RoundResult:
     return PreemptingQueueScheduler(inp, device).schedule()
 
 
+def _gang_csr(gangs):
+    """A dry-run call's gangs (lists of job-class indices) as CSR arrays: member offsets, members, and a
+    cleared ok per gang and node per member for the library to fill."""
+    import numpy as np
+    start = np.zeros(len(gangs) + 1, np.uint32)
+    start[1:] = np.cumsum([len(g) for g in gangs])
+    members = np.asarray([c for g in gangs for c in g] or [0], dtype=np.uint32)
+    ok = np.zeros(max(len(gangs), 1), np.uint8)
+    node = np.full(max(int(start[-1]), 1), abi.NONE, np.uint32)
+    return start, members, ok, node
+
+
 class DeviceNodeDb:
     """`NodeDb` on an empty cluster for dry-run gang checks — what SubmitChecker builds per executor
     (internal/scheduler/submitcheck.go:302-422).  `schedule_many(gangs)` = one
@@ -103,21 +113,12 @@ class DeviceNodeDb:
         self.lib = lib if lib is not None else abi.load_product()
         self.h = C.c_void_p()
         self._input = inp
-        st = self.lib.armada_nodedb_create(device, C.byref(inp), C.byref(self.h))
-        if st != abi.OK:
-            raise abi.ArmadaError(st, f"{self.lib.armada_strerror(st).decode()}: {self.lib.armada_last_error().decode()}")
+        _check(self.lib, self.lib.armada_nodedb_create(device, C.byref(inp), C.byref(self.h)))
 
     def schedule_many(self, gangs):
-        import numpy as np
-        start = np.zeros(len(gangs) + 1, np.uint32)
-        start[1:] = np.cumsum([len(g) for g in gangs])
-        members = np.asarray([c for g in gangs for c in g] or [0], dtype=np.uint32)
-        ok = np.zeros(max(len(gangs), 1), np.uint8)
-        node = np.full(max(int(start[-1]), 1), abi.NONE, np.uint32)
-        st = self.lib.armada_nodedb_schedule_many(self.h, len(gangs), start.ctypes.data_as(abi.u32p), members.ctypes.data_as(abi.u32p),
-                                                  ok.ctypes.data_as(abi.u8p), node.ctypes.data_as(abi.u32p))
-        if st != abi.OK:
-            raise abi.ArmadaError(st, f"{self.lib.armada_strerror(st).decode()}: {self.lib.armada_last_error().decode()}")
+        start, members, ok, node = _gang_csr(gangs)
+        _check(self.lib, self.lib.armada_nodedb_schedule_many(self.h, len(gangs), start.ctypes.data_as(abi.u32p), members.ctypes.data_as(abi.u32p),
+                                                              ok.ctypes.data_as(abi.u8p), node.ctypes.data_as(abi.u32p)))
         out_nodes = [node[int(start[g]):int(start[g + 1])].copy() for g in range(len(gangs))]
         return ok[: len(gangs)].astype(bool), out_nodes
 
@@ -129,11 +130,7 @@ class DeviceNodeDb:
         `capacity` and is grown once, to the size the library reports, when it was too small."""
         import numpy as np
         G = len(gangs)
-        start = np.zeros(G + 1, np.uint32)
-        start[1:] = np.cumsum([len(g) for g in gangs])
-        members = np.asarray([c for g in gangs for c in g] or [0], dtype=np.uint32)
-        ok = np.zeros(max(G, 1), np.uint8)
-        node = np.full(max(int(start[-1]), 1), abi.NONE, np.uint32)
+        start, members, ok, node = _gang_csr(gangs)
         placed = np.zeros(max(G, 1), np.uint32)
         away = np.zeros(max(G, 1), np.uint8)
         rstart = np.zeros(G + 1, np.uint32)
@@ -141,11 +138,9 @@ class DeviceNodeDb:
         cap = max(int(capacity), 1)
         for _ in range(2):
             recs = (abi.ExcludedReason * cap)()
-            st = self.lib.armada_nodedb_explain(self.h, G, start.ctypes.data_as(abi.u32p), members.ctypes.data_as(abi.u32p), ok.ctypes.data_as(abi.u8p),
-                                                node.ctypes.data_as(abi.u32p), placed.ctypes.data_as(abi.u32p), away.ctypes.data_as(abi.u8p),
-                                                rstart.ctypes.data_as(abi.u32p), recs, cap, C.byref(needed))
-            if st != abi.OK:
-                raise abi.ArmadaError(st, f"{self.lib.armada_strerror(st).decode()}: {self.lib.armada_last_error().decode()}")
+            _check(self.lib, self.lib.armada_nodedb_explain(self.h, G, start.ctypes.data_as(abi.u32p), members.ctypes.data_as(abi.u32p),
+                                                            ok.ctypes.data_as(abi.u8p), node.ctypes.data_as(abi.u32p), placed.ctypes.data_as(abi.u32p),
+                                                            away.ctypes.data_as(abi.u8p), rstart.ctypes.data_as(abi.u32p), recs, cap, C.byref(needed)))
             if needed.value <= cap:
                 break
             cap = needed.value
@@ -164,9 +159,7 @@ class DeviceNodeDb:
         import numpy as np
         cls = np.asarray(list(classes) or [0], dtype=np.uint32)
         node = np.full(len(cls), abi.NONE, np.uint32)
-        st = self.lib.armada_nodedb_select_nodes(self.h, len(list(classes)), cls.ctypes.data_as(abi.u32p), node.ctypes.data_as(abi.u32p))
-        if st != abi.OK:
-            raise abi.ArmadaError(st, f"{self.lib.armada_strerror(st).decode()}: {self.lib.armada_last_error().decode()}")
+        _check(self.lib, self.lib.armada_nodedb_select_nodes(self.h, len(list(classes)), cls.ctypes.data_as(abi.u32p), node.ctypes.data_as(abi.u32p)))
         return node[: len(list(classes))]
 
     def add_classes(self, class_request, class_pc, class_static_row, class_away_row, static_match, type_match) -> int:
@@ -192,10 +185,9 @@ class DeviceNodeDb:
         valid = np.ones(max(n, 1), np.uint8)
         first = C.c_uint32(0)
         ptr = lambda a, t: a.ctypes.data_as(t) if a.size else None  # noqa: E731
-        st = self.lib.armada_nodedb_add_classes(self.h, n, ptr(req.reshape(-1), abi.i64p), ptr(pc, abi.u32p), ptr(row, abi.u32p), ptr(away.reshape(-1), abi.u32p),
-                                                valid.ctypes.data_as(abi.u8p), len(sm), ptr(sm, abi.u32p), ptr(tm, abi.u32p), C.byref(first))
-        if st != abi.OK:
-            raise abi.ArmadaError(st, f"{self.lib.armada_strerror(st).decode()}: {self.lib.armada_last_error().decode()}")
+        _check(self.lib, self.lib.armada_nodedb_add_classes(self.h, n, ptr(req.reshape(-1), abi.i64p), ptr(pc, abi.u32p), ptr(row, abi.u32p),
+                                                            ptr(away.reshape(-1), abi.u32p), valid.ctypes.data_as(abi.u8p), len(sm), ptr(sm, abi.u32p),
+                                                            ptr(tm, abi.u32p), C.byref(first)))
         return first.value
 
     def close(self):

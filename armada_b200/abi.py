@@ -186,6 +186,17 @@ class RoundStats(C.Structure):
     ]
 
 
+# Elements of the RoundStats arrays read by name (their meanings: include/armada_b200.h)
+PHASE_BATCH_ITERATIONS = 4  # phase_cycles: loop iterations run in batch mode (a count, not cycles)
+BATCH_COUNT = 6             # batch_cycles: batches (a count, not cycles)
+DEBUG_PIPELINE_RUNS = 2     # batch_debug: pipeline runs
+DEBUG_BATCHES_CUT = 3       # batch_debug: batches cut short
+DEBUG_SLOW_STEPS = 4        # batch_debug: slow steps of the assignment loop, then their cycles
+DEBUG_SLOW_CYCLES = 5
+DEBUG_REFILLS = 6           # batch_debug: candidate refills from the sorted index, then their cycles
+DEBUG_REFILL_CYCLES = 7
+
+
 class ExcludedReason(C.Structure):
     _fields_ = [
         ("kind", C.c_uint32),

@@ -26,24 +26,70 @@
 #define ARMADA_DEV_MAX_SLOTS 22  // best-fit index slots: 2 per owning index warp (11 owners; batch mode keeps both in registers)
 #define ARMADA_DEV_VARIANTS (1 + ARMADA_MAX_AWAY)  // home + away node types per class
 
-// Slots of DevPtrs::stats: counters summed over the schedule passes of a round (k_reset zeroes them; the host
-// reads them into ArmadaRoundStats and the ARMADA_PRINT_STATS lines).  A group of n slots starts at its base.
+// Slots of the schedule pass's counters (SmemHdr::stat, summed into DevPtrs::stats over the passes of a round;
+// k_reset zeroes them; the host reads them into ArmadaRoundStats and the ARMADA_PRINT_STATS lines).  Cycles are SM
+// clock cycles.  Index warp 0 writes the batch_cycles slots but STAT_BT_CONTROL, and STAT_BT_CUT; the index warps add
+// STAT_RESCANS atomically; the control warp writes the others.
 enum StatSlot {
-  STAT_ITERS = 0,       // loop iterations
-  STAT_PROBES = 1,
-  STAT_PLACEMENTS = 2,
-  STAT_FAIR = 3,        // fair-preemption scans
-  STAT_RESCANS = 4,     // ArmadaRoundStats::tree_rescans
-  STAT_KERNEL = 5,      // control-warp cycles: the whole kernel
-  STAT_STARTUP = 6,     // … before the loop
-  STAT_RUNS = 7,        // … in pipeline runs
-  STAT_PROF = 8,        // [8] ArmadaRoundStats::phase_cycles
-  STAT_BT_CYC = 16,     // [8] ArmadaRoundStats::batch_cycles
-  STAT_BT_DBG = 24,     // [8] ArmadaRoundStats::batch_debug
-  STAT_TL = 32,         // [8] control-warp timeline
-  STAT_GL = 40,         // [8] general-loop timeline
-  STAT_GATE = 48,       // [2] level-0 miss gate probes: run, skipped
-  STAT_COUNT = 50,
+  STAT_ITERS = 0,          // loop iterations (the general loop's and the batched ones)
+  STAT_PROBES = 1,         // SelectNode index walks
+  STAT_PLACEMENTS = 2,     // successful binds
+  STAT_FAIR = 3,           // fair-preemption scans
+  STAT_RESCANS = 4,        // ArmadaRoundStats::tree_rescans: windows refilled from scratch
+  STAT_KERNEL = 5,         // control-warp cycles: the whole kernel
+  STAT_STARTUP = 6,        // … before the loop
+  STAT_RUNS = 7,           // … in pipeline runs (Ctl::run_batch)
+  // ArmadaRoundStats::phase_cycles: control-warp cycles in the general loop
+  STAT_PROF = 8,
+  STAT_PROF_PQ_TOP = 8,    // queue arg-min
+  STAT_PROF_GANG = 9,      // gang bookkeeping and constraints (the whole gang_schedule)
+  STAT_PROF_SELECT = 10,   // node selection
+  STAT_PROF_BIND = 11,     // node row update
+  STAT_BATCH_ITERS = 12,   // loop iterations run in batch mode (a count)
+  STAT_PROF_RESULT = 13,   // result algebra
+  STAT_PROF_ADVANCE = 14,  // iterator advance (it_peek)
+  STAT_PROF_CLEAR = 15,    // cost update (candidate_clear)
+  // ArmadaRoundStats::batch_cycles: index-warp cycles of the batch pipeline
+  STAT_BT_CYC = 16,
+  STAT_BT_BUILD = 16,      // item build
+  STAT_BT_HORIZON = 17,    // horizon
+  STAT_BT_RANK = 18,       // merge ranks and speculative advance
+  STAT_BT_WAIT = 19,       // waiting for the assignment loop
+  STAT_BT_COMMIT = 20,     // apply and commit
+  STAT_BT_CONTROL = 21,    // control warp: bookkeeping after a pipeline run
+  STAT_BT_BATCHES = 22,    // batches (a count)
+  STAT_BT_EPILOGUE = 23,   // pipeline epilogue
+  // ArmadaRoundStats::batch_debug: the assignment loop
+  STAT_BT_DBG = 24,
+  STAT_CHAIN_BUSY = 24,    // cycles busy
+  STAT_CHAIN_WAIT = 25,    // cycles waiting for records
+  STAT_PIPELINE_RUNS = 26, // pipeline runs
+  STAT_BT_CUT = 27,        // batches cut short
+  STAT_SLOW_STEPS = 28,    // slow steps (ensure_groups; chain_swar only)
+  STAT_SLOW_CYCLES = 29,   // … their cycles
+  STAT_REFILLS = 30,       // candidate refills from the G0 cursor (chain_swar only)
+  STAT_REFILL_CYCLES = 31, // … their cycles
+  // control-warp timeline (ARMADA_PRINT_STATS)
+  STAT_TL_PRECREATE = 32,         // creating windows up front
+  STAT_TL_FIRST_BATCH_WAIT = 33,  // waiting for the first batch of a run
+  STAT_TL_AFTER_CHAIN_WAIT = 34,  // waiting for the index warps after the assignment loop
+  STAT_TL_FAILED_ITERS = 35,      // general iterations that failed
+  STAT_TL_FAILED_CYCLES = 36,     // … their cycles
+  STAT_TL_FAIR_QUERY = 37,        // fair-preemption queries
+  STAT_TL_LEVEL_SCAN = 38,        // level scans
+  STAT_TL_EVICTED_REBIND = 39,    // re-binds of evicted single jobs
+  // general-loop timeline (ARMADA_PRINT_STATS)
+  STAT_GL_WAIT_INDEX = 40,     // waiting for the index warps (wait_consumed)
+  STAT_GL_RING_FULL = 41,      // message ring full (post)
+  STAT_GL_SELECT_QUEUED = 42,  // node selection of queued jobs
+  STAT_GL_BIND_QUEUED = 43,    // their binds
+  STAT_GL_FAIR_VICTIMS = 44,   // victims of fair preemption
+  STAT_GL_PROLOGUE = 45,       // iteration prologue (members, accounting, constraints)
+  STAT_GL_SELECT_COUNT = 46,   // node selections of queued jobs (a count)
+  // fast domain, after a level-0 miss: gate probes at the job's own level
+  STAT_GATE_RUN = 47,      // … that ran
+  STAT_GATE_SKIPPED = 48,  // … skipped (final miss)
+  STAT_COUNT = 49,
 };
 
 // Slots of DevPtrs::s_counts: the round's sctx counts, carried from kernel to kernel (k_reset sets them; the schedule

@@ -122,7 +122,7 @@ def fast_domain_batch(dev, capfd, D, seed, excl=False, derive=False, n_nodes=60)
     assert form in ("k32", "k64"), f"{r.name}: the library chose {form} ({lay})"
     bad = got.diff(want)
     assert not bad, f"{r.name}: device != oracle:\n  " + "\n  ".join(bad)
-    assert int(got.stats.phase_cycles[4]) > 0, "expected batch-mode iterations"
+    assert int(got.stats.phase_cycles[abi.PHASE_BATCH_ITERATIONS]) > 0, "expected batch-mode iterations"
     # non-preemptible jobs hold the rows: still negative at level 0 when the round ends
     assert (np.asarray(want.node_alloc)[0] < 0).any()
     if excl:
@@ -162,7 +162,7 @@ def unindexed_negative(schedule, seed, n_nodes=60, n_jobs=500):
     # … and still no new job lands there
     new = (np.asarray(r.job_node).astype(np.int64) == abi.NONE) & (st == abi.JOB_SCHEDULED)
     assert not np.isin(jn[new], neg).any()
-    assert int(got.stats.phase_cycles[4]) > 0
+    assert int(got.stats.phase_cycles[abi.PHASE_BATCH_ITERATIONS]) > 0
     assert _failed_job_counts_resources(want)
 
 

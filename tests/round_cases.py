@@ -91,7 +91,7 @@ def partly_indexed_resources(schedule, seed, indexed):
     r.indexed = indexed
     got, _ = assert_parity(schedule, r.to_input(), f"{r.name} indexed={indexed}")
     if batchy:
-        assert int(got.stats.phase_cycles[4]) > 0
+        assert int(got.stats.phase_cycles[abi.PHASE_BATCH_ITERATIONS]) > 0
 
 
 def exact_mode_unaligned_round(schedule, seed):

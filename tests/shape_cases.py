@@ -300,7 +300,7 @@ def check_case(case: Case, dev, oracle_round, capfd):
     bad = got.diff(want)
     assert not bad, f"{case.id}: device != oracle:\n  " + "\n  ".join(bad)
     if case.kind == "batch" and case.form != "exact" and case.n_nodes >= 32:  # (1–2 nodes may fill up before a batch)
-        assert int(got.stats.phase_cycles[4]) > 0, "expected batch-mode iterations"
+        assert int(got.stats.phase_cycles[abi.PHASE_BATCH_ITERATIONS]) > 0, "expected batch-mode iterations"
     if case.form == "run" and case.kind == "batch":
         ex = np.asarray(want.job_excluded_nodes)
         assert ex[:, abi.EXCL_RESOURCES].sum() > 0, "the unindexed extras never rejected a reached node"
@@ -401,7 +401,7 @@ def long_batch_pipeline(make_dev, wq, seed):
         bad = got.diff(want)
         assert not bad, f"{r.name}: device != oracle:\n  " + "\n  ".join(bad)
         if seed != 503:
-            assert int(got.stats.batch_cycles[6]) >= {500: 8, 501: 2, 502: 3}[seed], "expected several batches per pipeline run"
+            assert int(got.stats.batch_cycles[abi.BATCH_COUNT]) >= {500: 8, 501: 2, 502: 3}[seed], "expected several batches per pipeline run"
         dev.close()
 
 
@@ -421,7 +421,7 @@ def gangs_as_batch_items(make_dev, nodes, queues, jobs, wq, seed):
         assert not bad, f"C4 {nodes}x{jobs}: device != oracle:\n  " + "\n  ".join(bad)
         # gang members were placed in batch mode: more placements than iterations there
         assert int(got.stats.placements) > int(got.stats.loop_iterations) - int(np.count_nonzero(np.asarray(want.job_state) == 4))
-        assert int(got.stats.phase_cycles[4]) > 0
+        assert int(got.stats.phase_cycles[abi.PHASE_BATCH_ITERATIONS]) > 0
         dev.close()
 
 

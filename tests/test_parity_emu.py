@@ -67,7 +67,7 @@ def test_many_queues(n_queues):
     a different power of two); priorities off so that most of the round runs in batch mode."""
     r = synth.random_round(300 + n_queues, n_nodes=300, n_queues=n_queues, n_jobs=2500, n_running=0, gangs=False, priorities=False)
     got, _ = assert_parity(r.to_input(), r.name)
-    assert int(got.stats.phase_cycles[4]) > 0
+    assert int(got.stats.phase_cycles[abi.PHASE_BATCH_ITERATIONS]) > 0
 
 
 @pytest.mark.parametrize("name,scale", [("C2", 0.02), ("C3", 0.004), ("C4", 0.006), ("C5", 0.004)])

@@ -79,7 +79,7 @@ def test_batch_mode_covers_the_plain_iterations_and_is_deterministic():
             ref = got
         else:
             assert not got.diff(ref)
-    assert int(st.phase_cycles[4]) > 0.8 * int(st.loop_iterations)
+    assert int(st.phase_cycles[abi.PHASE_BATCH_ITERATIONS]) > 0.8 * int(st.loop_iterations)
     want = oracle_lib.round_schedule(inp)
     assert not ref.diff(want)
 
@@ -309,7 +309,7 @@ def test_shape_rounds_are_deterministic(case):
                 ref = got
             else:
                 assert not got.diff(ref)
-    assert int(st.phase_cycles[4]) > 0
+    assert int(st.phase_cycles[abi.PHASE_BATCH_ITERATIONS]) > 0
     assert not ref.diff(oracle_lib.round_schedule(inp))
 
 

@@ -6,7 +6,7 @@ import sys
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
-from armada_b200 import synth  # noqa: E402
+from armada_b200 import abi, synth  # noqa: E402
 from armada_b200.scheduler import DeviceRound  # noqa: E402
 
 
@@ -26,15 +26,15 @@ with DeviceRound(0) as dev:
             st = dev.run()
             if best is None or st.device_ms < best.device_ms:
                 best = st
-        it = max(1, int(best.phase_cycles[4]))
+        it = max(1, int(best.phase_cycles[abi.PHASE_BATCH_ITERATIONS]))
         print(json.dumps({"config": name, "device_ms": round(best.device_ms, 3), "pass_ms": round(best.schedule_pass_ms, 3),
                           "placements": int(best.placements), "iterations": int(best.loop_iterations),
-                          "batched": int(best.phase_cycles[4]), "batches": int(best.batch_cycles[6]),
+                          "batched": int(best.phase_cycles[abi.PHASE_BATCH_ITERATIONS]), "batches": int(best.batch_cycles[abi.BATCH_COUNT]),
                           "placements_per_s": round(best.placements / (best.device_ms / 1e3)),
                           "batch_cycles_per_iter": [round(int(best.batch_cycles[i]) / it, 1) for i in range(6)],
-                          "chain_busy_wait_per_iter": [round(int(best.batch_debug[i]) / it, 1) for i in range(2)], "runs_cut": [int(best.batch_debug[2]), int(best.batch_debug[3])],
-                          "slow_steps": int(best.batch_debug[4]), "cycles_per_slow_step": round(int(best.batch_debug[5]) / max(1, int(best.batch_debug[4]))),
-                          "refills": int(best.batch_debug[6]), "cycles_per_refill": round(int(best.batch_debug[7]) / max(1, int(best.batch_debug[6]))),
+                          "chain_busy_wait_per_iter": [round(int(best.batch_debug[i]) / it, 1) for i in range(2)], "runs_cut": [int(best.batch_debug[abi.DEBUG_PIPELINE_RUNS]), int(best.batch_debug[abi.DEBUG_BATCHES_CUT])],
+                          "slow_steps": int(best.batch_debug[abi.DEBUG_SLOW_STEPS]), "cycles_per_slow_step": round(int(best.batch_debug[abi.DEBUG_SLOW_CYCLES]) / max(1, int(best.batch_debug[abi.DEBUG_SLOW_STEPS]))),
+                          "refills": int(best.batch_debug[abi.DEBUG_REFILLS]), "cycles_per_refill": round(int(best.batch_debug[abi.DEBUG_REFILL_CYCLES]) / max(1, int(best.batch_debug[abi.DEBUG_REFILLS]))),
                           "fair_scans": int(best.fair_preemption_scans), "ev1": int(best.evicted_pass1), "ev2": int(best.evicted_pass2),
                           "probes": int(best.probes), "rescans": int(best.tree_rescans),
                           "phase_mcycles": [round(int(best.phase_cycles[i]) / 1e6, 1) for i in range(8)]}), flush=True)

@@ -73,8 +73,8 @@ enum StatSlot {
   STAT_TL_PRECREATE = 32,         // creating windows up front
   STAT_TL_FIRST_BATCH_WAIT = 33,  // waiting for the first batch of a run
   STAT_TL_AFTER_CHAIN_WAIT = 34,  // waiting for the index warps after the assignment loop
-  STAT_TL_FAILED_ITERS = 35,      // general iterations that failed
-  STAT_TL_FAILED_CYCLES = 36,     // … their cycles
+  STAT_TL_FAILED_ITERS = 35,      // loop iterations that failed (STAT_BT_FAILS of them in the batch pipeline)
+  STAT_TL_FAILED_CYCLES = 36,     // … the cycles of those in the general loop
   STAT_TL_FAIR_QUERY = 37,        // fair-preemption queries
   STAT_TL_LEVEL_SCAN = 38,        // level scans
   STAT_TL_EVICTED_REBIND = 39,    // re-binds of evicted single jobs
@@ -89,7 +89,8 @@ enum StatSlot {
   // fast domain, after a level-0 miss: gate probes at the job's own level
   STAT_GATE_RUN = 47,      // … that ran
   STAT_GATE_SKIPPED = 48,  // … skipped (final miss)
-  STAT_COUNT = 49,
+  STAT_BT_FAILS = 49,      // jobs the batch pipeline failed (their level-0 miss final, Ctl::level0_miss_final)
+  STAT_COUNT = 50,
 };
 
 // Slots of DevPtrs::s_counts: the round's sctx counts, carried from kernel to kernel (k_reset sets them; the schedule

@@ -27,6 +27,7 @@ from . import abi
 UNSCHEDULABLE_TAINT_KEY = "armadaproject.io/unschedulable"  # internaltypes/unschedulable.go:7-17
 NODE_ID_LABEL = "armadaproject.io/nodeId"
 WILDCARD = "*"  # configuration.WildCardWellKnownNodeTypeValue
+PODS = "pods"  # armadaresource.PodsResourceName: the node's pod capacity (node.Status.Allocatable["pods"])
 
 _SUFFIX = {
     "": Fraction(1), "n": Fraction(1, 10**9), "u": Fraction(1, 10**6), "m": Fraction(1, 1000), "k": Fraction(10**3), "M": Fraction(10**6), "G": Fraction(10**9),
@@ -208,6 +209,14 @@ class SchedulingConfig:
     disallowed_resources: Sequence[str] = ()
     # FloatingResources of THIS pool (configuration.FloatingResourceConfig): resources no node holds, limited per pool
     floating_resources: Sequence["FloatingResource"] = ()
+    # RespectNodePodLimits (configuration.go:227): every job is one pod, counted against each node's `pods` capacity.
+    # Takes effect once apply_respect_node_pod_limits has added `pods` to the resource lists.
+    respect_node_pod_limits: bool = False
+
+    def job_requests(self, requests: Dict[str, object]) -> Dict[str, object]:
+        """A job's requests as the JobDb records them (getResourceRequirements, jobdb.go:256-263): with
+        respect_node_pod_limits the job asks for one pod, whatever its own requests say about pods."""
+        return {**requests, PODS: 1} if self.respect_node_pod_limits else requests
 
     def factory(self) -> ResourceListFactory:
         # NewResourceListFactory: the supported (Kubernetes) types, then the floating ones (resource_list_factory.go:41-53)
@@ -221,6 +230,28 @@ class SchedulingConfig:
             for a in pc.away_node_types:
                 ps.add(a.priority)
         return sorted(ps)
+
+
+def apply_respect_node_pod_limits(cfg: SchedulingConfig) -> bool:
+    """ApplyRespectNodePodLimits (configuration.go:548-580): with the knob on, `pods` at resolution 1 becomes a
+    supported and an indexed resource, so that the factory, the NodeDb's index and every resource list count pods.
+    An existing `pods` entry is reset to resolution 1 in place (each job is exactly one pod slot); otherwise the
+    entry is appended.  Idempotent; returns whether the knob is on (and the config was brought to that form).
+    Call it before the config makes a factory, a builder, a SubmitChecker or a Simulator."""
+    if not cfg.respect_node_pod_limits:
+        return False
+
+    def ensure(types: Sequence[ResourceType]) -> List[ResourceType]:  # ensurePodsResourceType
+        out = list(types)
+        for i, t in enumerate(out):
+            if t.name == PODS:
+                out[i] = ResourceType(PODS, "1")
+                return out
+        return out + [ResourceType(PODS, "1")]
+
+    cfg.supported_resource_types = ensure(cfg.supported_resource_types)
+    cfg.indexed_resources = ensure(cfg.indexed_resources)
+    return True
 
 
 @dataclass
@@ -429,7 +460,7 @@ class RoundInputBuilder:
         cfg, f = self.cfg, self.factory
         job_class = np.zeros(len(jobs), dtype=np.uint32)
         for ji, j in enumerate(jobs):
-            req = f.from_job(j.requests)
+            req = f.from_job(cfg.job_requests(j.requests))
             key = scheduling_key(j, req)
             if key not in self._classes:
                 self._classes[key] = len(self._class_req)

@@ -35,7 +35,7 @@ import numpy as np
 
 from . import abi
 from .model import (AwayNodeType, JobSpec, NodeSpec, PriorityClass, QueueSpec, ResourceType, RoundInputBuilder, RoundResult,
-                    SchedulingConfig, Taint, Toleration, parse_quantity)
+                    SchedulingConfig, Taint, Toleration, apply_respect_node_pod_limits, parse_quantity)
 
 CLUSTER_LABEL = "armadaproject.io/clusterName"  # simulator.go:45
 NS = 1_000_000_000
@@ -245,7 +245,7 @@ def scheduling_config_from_dict(d: dict) -> Tuple[SchedulingConfig, str]:
         maximum_per_queue_scheduling_rate=rate(g("maximumPerQueueSchedulingRate"), math.inf),
         maximum_per_queue_scheduling_burst=int(g("maximumPerQueueSchedulingBurst", 2**62)),
         enable_prefer_large_job_ordering=bool(g("enablePreferLargeJobOrdering", False)),
-        disallowed_resources=())
+        disallowed_resources=(), respect_node_pod_limits=bool(g("respectNodePodLimits", False)))
     return cfg, str(g("defaultPriorityClassName", ""))
 
 
@@ -442,6 +442,7 @@ class Simulator:
         self.enable_fast_forward = enable_fast_forward
         self.hard_termination_ns = hard_termination_minutes * 60 * NS
         self.period_ns = scheduler_cycle_period_seconds * NS
+        apply_respect_node_pod_limits(self.cfg)  # NewSimulator (simulator.go:123), before the factory is made
         self.factory = scheduling_config.factory()
         self.time = 0  # epochStart
         self.seq = 0
@@ -643,7 +644,7 @@ class Simulator:
 
     # -- event sequences -----------------------------------------------------------------------
     def _req_vector(self, t: JobTemplate) -> np.ndarray:
-        return self.factory.from_job(t.requests)
+        return self.factory.from_job(self.cfg.job_requests(t.requests))
 
     def _row(self, j: _Job, state: str) -> JobRunRow:
         t = j.template

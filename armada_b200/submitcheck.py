@@ -260,7 +260,7 @@ class SubmitChecker:
         single = [copy.copy(j) for j in jobs]
         for j in single:  # getIndividualSchedulingResult strips the gang info (:270-271); it plays no part in a job's class
             j.gang_id, j.gang_cardinality = None, 1
-        keys = [scheduling_key(j, self.factory.from_job(j.requests)) for j in single]
+        keys = [scheduling_key(j, self.factory.from_job(self.cfg.job_requests(j.requests))) for j in single]
         job_class = {key: self._register(key, single) for key in list(self.dbs)}
         by_queue: Dict[str, List[int]] = {}
         gangs: Dict[Tuple[str, str], List[int]] = {}
@@ -325,7 +325,7 @@ class SubmitChecker:
     def _scheduling_result(self, members: List[int], k: int, jobs, dry, job_class) -> SchedulingResult:
         """getSchedulingResult (:302-422) of one item: the k-th of the launch `dry`."""
         f = self.factory
-        req = np.sum([f.from_job(jobs[i].requests) for i in members], axis=0)
+        req = np.sum([f.from_job(self.cfg.job_requests(jobs[i].requests)) for i in members], axis=0)
         floating_req = np.asarray([req[d] if f.names[d] in self.floating else 0 for d in range(f.D)], np.int64)
         first = jobs[members[0]]
         successful: List[str] = []

@@ -323,6 +323,31 @@ def config_c5(n_nodes=100_000, n_queues=64, n_new_jobs=400_000, seed=SEED) -> Ra
         queue_weight=_weights(n_queues), protected_fraction=0.5, name="C5")
 
 
+def with_pod_limits(r: RawRound, pods) -> RawRound:
+    """`r` with RespectNodePodLimits on (model.apply_respect_node_pod_limits): a `pods` resource after the others,
+    indexed last at resolution 1, `pods` per node (a number or one per node) and one pod per job.  Pods play no part
+    in DRF (they are not among its resources) and have no round or queue limit.  A node never starts above its pod
+    capacity: one with more running jobs than `pods` gets a capacity of its running jobs."""
+    D, N = r.node_total.shape
+    cap = np.broadcast_to(np.asarray(pods, np.int64), (N,)).copy()
+    if r.job_node is not None:
+        jn = np.asarray(r.job_node).astype(np.int64)
+        cap = np.maximum(cap, np.bincount(jn[jn != abi.NONE], minlength=N)[:N])
+    indexed = list(r.indexed) if r.indexed is not None else list(INDEXED)
+    res = list(r.resolution) if r.resolution is not None else [RESOLUTION[INDEXED.index(d)] for d in indexed]
+    drf = list(r.drf_multipliers) if r.drf_multipliers is not None else [1.0] * D
+    r.node_total = np.vstack([r.node_total, cap[None, :]])
+    r.node_allocatable = np.vstack([r.node_allocatable, cap[None, :]])
+    r.class_request = np.hstack([np.asarray(r.class_request, np.int64), np.ones((len(r.class_request), 1), np.int64)])
+    r.indexed, r.resolution, r.drf_multipliers = indexed + [D], res + [1], drf + [0.0]
+    if r.round_limit is not None:
+        r.round_limit = np.append(r.round_limit, I64_MAX)
+    if r.queue_limit is not None:
+        r.queue_limit = np.concatenate([r.queue_limit, np.full(r.queue_limit.shape[:2] + (1,), I64_MAX, np.int64)], axis=2)
+    r.name += "+pods"
+    return r
+
+
 def unfeasible_runs_round(n_nodes: int) -> RawRound:
     """Edge case: runs of jobs whose scheduling key is already known to be unfeasible
     (queue_scheduler.go:339-349), shorter and longer than the iterator's 128-record fast-forward

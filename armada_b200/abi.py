@@ -36,6 +36,7 @@ LABEL_NOT_INDEXED = 0xFFFFFFFE
 
 NODE_UNSCHEDULABLE = 1
 NODE_OVERALLOCATED = 2
+NODE_DROPPED = 4  # armada_round_download_snapshot only: the node is not in the NodeDb
 
 u8p = C.POINTER(C.c_uint8)
 u32p = C.POINTER(C.c_uint32)
@@ -138,6 +139,21 @@ class RoundInput(C.Structure):
         ("floating_limits_configured", C.c_uint8),
         ("_pad_floating", C.c_uint8 * 3),
         ("floating_limit", C.c_int64 * MAX_RESOURCES),
+    ]
+
+
+class ClusterState(C.Structure):
+    """ArmadaClusterState: the pool as reported, for armada_round_upload_cluster."""
+    _fields_ = [
+        ("abi_version", C.c_uint32),
+        ("num_other_pool_jobs", C.c_uint32),
+        ("other_pool_job_node", u32p),
+        ("other_pool_job_request", i64p),
+        ("static_class_unschedulable", u32p),
+        ("has_round_limit", C.c_uint8),
+        ("_pad", C.c_uint8 * 7),
+        ("max_fraction_to_schedule", C.c_double * MAX_RESOURCES),
+        ("queue_limit_fraction", f64p),
     ]
 
 
@@ -245,6 +261,10 @@ def declare_prototypes(lib: C.CDLL) -> None:
     lib.armada_round_create.restype = C.c_int32
     lib.armada_round_upload.argtypes = [vp, C.POINTER(RoundInput)]
     lib.armada_round_upload.restype = C.c_int32
+    lib.armada_round_upload_cluster.argtypes = [vp, C.POINTER(RoundInput), C.POINTER(ClusterState)]
+    lib.armada_round_upload_cluster.restype = C.c_int32
+    lib.armada_round_download_snapshot.argtypes = [vp, u8p, i64p, u32p, i64p, i64p, i64p]
+    lib.armada_round_download_snapshot.restype = C.c_int32
     lib.armada_round_run.argtypes = [vp, C.POINTER(RoundStats)]
     lib.armada_round_run.restype = C.c_int32
     lib.armada_round_run_deadline.argtypes = [vp, C.POINTER(RoundStats), C.c_uint64]
@@ -293,6 +313,8 @@ def load_product() -> C.CDLL:
 PRODUCT_SYMBOLS = [
     "armada_round_create",
     "armada_round_upload",
+    "armada_round_upload_cluster",
+    "armada_round_download_snapshot",
     "armada_round_run",
     "armada_round_run_deadline",
     "armada_round_download",

@@ -613,4 +613,5 @@ __global__ void k_finalize(DevCfg c, DevPtrs P, uint8_t* out_state, uint32_t* ou
 }  // namespace
 
 #include "armada_dryrun.inc"
+#include "armada_snapshot.inc"
 #include "armada_host.inc"

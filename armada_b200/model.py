@@ -14,9 +14,10 @@ The string logic runs on the host; the device only sees dense ids and bitmaps.
 """
 from __future__ import annotations
 
+import ctypes
 import math
 import operator
-from dataclasses import dataclass, field
+from dataclasses import dataclass, field, replace
 from fractions import Fraction
 from typing import Dict, List, Optional, Sequence, Tuple
 
@@ -264,6 +265,9 @@ class NodeSpec:
     allocatable: Optional[Dict[str, object]] = None  # default: total
     unschedulable: bool = False
     over_allocated: bool = False
+    # whether the node type was made with the unschedulable taint (None: as `unschedulable` says).  A node that
+    # populateNodeDb marks unschedulable keeps the type it was created with (WithSchedulable, node.go:302-310).
+    type_unschedulable: Optional[bool] = None
 
 
 @dataclass
@@ -313,6 +317,71 @@ def multiply_resource(res: int, m: float) -> int:
     return int(v)
 
 
+def _kubernetes_requirements(cfg: SchedulingConfig, f: "ResourceListFactory", requests) -> np.ndarray:
+    """Job.KubernetesResourceRequirements in factory units: the floating resources left out."""
+    req = f.from_job(cfg.job_requests(requests))
+    for fr in cfg.floating_resources:
+        req[f.index[fr.name]] = 0
+    return req
+
+
+def queue_limit_fractions(cfg: SchedulingConfig, pc_name: str, q: "QueueSpec") -> Dict[str, float]:
+    """calculatePerQueueLimits' fractions of one (queue, priority class), constraints.go:231-256."""
+    fractions = dict(cfg.priority_classes[pc_name].maximum_resource_fraction_per_queue)
+    fractions.update(q.resource_limits_by_pc.get(pc_name, {}))
+    return fractions
+
+
+def populate_node_db(cfg: SchedulingConfig, nodes: Sequence[NodeSpec], jobs: Sequence[JobSpec], other_pool_jobs: Sequence[JobSpec],
+                     queues: Sequence["QueueSpec"] = ()):
+    """populateNodeDb (scheduling_algo.go:861-935), the pool's total (:455-456) and NewSchedulingConstraints
+    (constraints/constraints.go:94-111, 205-256) on the specs of a pool as reported.  `jobs` are this pool's, `other_pool_jobs`
+    the other pools' (running ones have `node` set; jobs on nodes outside `nodes` are skipped).  Returns
+    (nodes, total, constraints): the NodeSpecs the NodeDb holds, in the given order — an unschedulable node without a job
+    of this pool is dropped; a node whose jobs Exceed its allocatable is over-allocated and unschedulable (keeping its node
+    type); the other pools' requests come off the allocatable, floored at zero — the total [D] (their allocatable plus the
+    floating totals), and {"max_resources_to_schedule": [D], "queue_limit": {queue: {priority class: [D]}}}."""
+    f = cfg.factory()
+    ids = {n.id for n in nodes}
+    pool_jobs: Dict[str, int] = {}
+    used: Dict[str, np.ndarray] = {}
+    other: Dict[str, np.ndarray] = {}
+    for j in jobs:
+        if j.node is None or j.node not in ids:
+            continue
+        pool_jobs[j.node] = pool_jobs.get(j.node, 0) + 1
+        used[j.node] = used.get(j.node, np.zeros(f.D, np.int64)) + _kubernetes_requirements(cfg, f, j.requests)
+    for j in other_pool_jobs:
+        if j.node is None or j.node not in ids:
+            continue
+        req = _kubernetes_requirements(cfg, f, j.requests)
+        used[j.node] = used.get(j.node, np.zeros(f.D, np.int64)) + req
+        other[j.node] = other.get(j.node, np.zeros(f.D, np.int64)) + req
+    kept: List[NodeSpec] = []
+    total = np.zeros(f.D, np.int64)
+    for n in nodes:
+        if n.unschedulable and not pool_jobs.get(n.id):
+            continue
+        alloc = f.from_node(n.allocatable if n.allocatable is not None else n.total)
+        m = replace(n, over_allocated=False)
+        if n.id in used and (used[n.id] > alloc).any():
+            m = replace(m, over_allocated=True, unschedulable=True, type_unschedulable=n.unschedulable)
+        if n.id in other:  # MarkResourceUnallocatable, node.go:285-294
+            alloc = np.maximum(alloc - other[n.id], 0)
+            m = replace(m, allocatable={name: Fraction(int(alloc[i])) * Fraction(10) ** f.scales[i] for i, name in enumerate(f.names)})
+        kept.append(m)
+        total += alloc
+    for fr in cfg.floating_resources:
+        if fr.quantity is not None:
+            total[f.index[fr.name]] += f.scaled_value(fr.name, fr.quantity)
+    fr = cfg.maximum_resource_fraction_to_schedule or {}
+    constraints = {"max_resources_to_schedule": np.array([multiply_resource(int(total[d]), fr.get(name, math.inf)) for d, name in enumerate(f.names)], np.int64),
+                   "queue_limit": {q.name: {pc: np.array([multiply_resource(int(total[d]), queue_limit_fractions(cfg, pc, q).get(name, math.inf))
+                                                          for d, name in enumerate(f.names)], np.int64) for pc in cfg.priority_classes}
+                                   for q in queues}}
+    return kept, total, constraints
+
+
 class UnresolvedLabels(ValueError):
     """RoundInputBuilder.add_jobs: a new row looks at a node label the builder's static classes do not resolve."""
 
@@ -333,8 +402,13 @@ class RoundInputBuilder:
 
     def __init__(self, cfg: SchedulingConfig, nodes: Sequence[NodeSpec], jobs: Sequence[JobSpec],
                  queues: Sequence[QueueSpec], total_resources: Optional[np.ndarray] = None,
-                 queued_order: Optional[Dict[str, List[str]]] = None, global_limiter_tokens: Optional[float] = None):
+                 queued_order: Optional[Dict[str, List[str]]] = None, global_limiter_tokens: Optional[float] = None,
+                 other_pool_jobs: Optional[Sequence[JobSpec]] = None):
+        """`other_pool_jobs` given (a list, possibly empty): the pool as reported, for armada_round_upload_cluster.  Then
+        `self.cluster_state` is its ArmadaClusterState; the nodes' over_allocated is not read, and every static class without
+        the unschedulable taint gets a variant with it (static_class_unschedulable), matched like the others."""
         self.cfg = cfg
+        self.other_pool_jobs = None if other_pool_jobs is None else list(other_pool_jobs)
         self.factory = cfg.factory()
         self.nodes = list(nodes)
         self.jobs = list(jobs)
@@ -359,6 +433,8 @@ class RoundInputBuilder:
         self._queues()  # the per-queue limits are fractions of _context's total_resources
         if queued_order is not None:
             self._queued_order(queued_order)
+        if self.other_pool_jobs is not None:
+            self._cluster_state()
 
     # -- helpers ---------------------------------------------------------------------------
     def _attach(self, **arrays):
@@ -596,7 +672,8 @@ class RoundInputBuilder:
                 static_specs.append((taints, labels))
             node_static[i] = static_classes[skey]
             # NewNodeType, node_type.go:68-124
-            ttaints = tuple(t for t in taints if indexed_taints is None or t.key in indexed_taints)
+            type_taints = taints if n.type_unschedulable is None else self._node_taints(replace(n, unschedulable=n.type_unschedulable))
+            ttaints = tuple(t for t in type_taints if indexed_taints is None or t.key in indexed_taints)
             tlabels = {k: v for k, v in labels.items() if k in indexed_labels}
             unset = set(k for k in indexed_labels if k not in tlabels)
             tkey = (tuple(sorted(ttaints, key=repr)), tuple(sorted(tlabels.items())), tuple(sorted(unset)))
@@ -607,7 +684,24 @@ class RoundInputBuilder:
                 types[tkey] = len(type_specs)
                 type_specs.append((ttaints, tlabels, unset))
             node_type[i] = types[tkey]
-            node_flags[i] = (abi.NODE_UNSCHEDULABLE if n.unschedulable else 0) | (abi.NODE_OVERALLOCATED if n.over_allocated else 0)
+            over = n.over_allocated and self.other_pool_jobs is None  # (the cluster path derives it)
+            node_flags[i] = (abi.NODE_UNSCHEDULABLE if n.unschedulable else 0) | (abi.NODE_OVERALLOCATED if over else 0)
+        self.static_class_unschedulable = None
+        if self.other_pool_jobs is not None:  # WithSchedulable(false): the class with the unschedulable taint added
+            unsched = Taint(UNSCHEDULABLE_TAINT_KEY, "true", "NoSchedule")
+            scu = []
+            for taints, labels in list(static_specs):
+                if any(t.key == UNSCHEDULABLE_TAINT_KEY for t in taints):
+                    scu.append(abi.NONE)
+                    continue
+                vt = tuple(taints) + (unsched,)
+                skey = (tuple(sorted(vt, key=repr)), tuple(sorted((k, v) for k, v in labels.items() if k in rel_keys)))
+                if skey not in static_classes:
+                    static_classes[skey] = len(static_specs)
+                    static_specs.append((vt, labels))
+                scu.append(static_classes[skey])
+            scu += [abi.NONE] * (len(static_specs) - len(scu))
+            self.static_class_unschedulable = scu
         inp.num_static_classes, inp.num_node_types = max(1, len(static_specs)), max(1, len(type_specs))
         self.static_specs, self.type_specs = static_specs, type_specs
         self.static_label_keys, self.node_label_keys = rel_keys, {k for n in self.nodes for k in self._node_labels(n)}
@@ -775,9 +869,8 @@ class RoundInputBuilder:
             if q.short_job_penalty is not None:
                 qp[i] = q.short_job_penalty
             # calculatePerQueueLimits, constraints.go:231-256
-            for pcn, pc in cfg.priority_classes.items():
-                fractions = dict(pc.maximum_resource_fraction_per_queue)
-                fractions.update(q.resource_limits_by_pc.get(pcn, {}))
+            for pcn in cfg.priority_classes:
+                fractions = queue_limit_fractions(cfg, pcn, q)
                 pi = self.pc_index[pcn]
                 qhl[i, pi] = 1
                 for d, name in enumerate(f.names):
@@ -788,6 +881,32 @@ class RoundInputBuilder:
         self._attach(queue_weight=qw, queue_cordoned=qc, queue_allocated_by_pc=qa, queue_demand=qd, queue_constrained_demand=qcd,
                      queue_short_job_penalty=qp, queue_has_limit=qhl, queue_limit=ql, queue_limiter_tokens=qt,
                      queue_limiter_burst=qb, queue_limiter_is_inf=qi)
+
+    def _cluster_state(self):
+        """ArmadaClusterState: the other pools' running jobs on this pool's nodes, the unschedulable variants of the
+        static classes and the caps of NewSchedulingConstraints as fractions (+Inf where none is configured)."""
+        cfg, f = self.cfg, self.factory
+        cs = abi.ClusterState()
+        cs.abi_version = abi.ABI_VERSION
+        on = [j for j in self.other_pool_jobs if j.node is not None and j.node in self.node_pos]
+        cs.num_other_pool_jobs = len(on)
+        fr = cfg.maximum_resource_fraction_to_schedule or {}
+        cs.has_round_limit = 1
+        for d, name in enumerate(f.names):
+            cs.max_fraction_to_schedule[d] = fr.get(name, math.inf)
+        qf = np.full((max(len(self.queues), 1), len(self.pc_names), f.D), math.inf)
+        for i, q in enumerate(self.queues):
+            for pcn in cfg.priority_classes:
+                fractions = queue_limit_fractions(cfg, pcn, q)
+                for d, name in enumerate(f.names):
+                    qf[i, self.pc_index[pcn], d] = fractions.get(name, math.inf)
+        self.cluster_keep: List[object] = []
+        self.cluster_state_arrays = abi.attach(
+            cs, self.cluster_keep, other_pool_job_node=[self.node_pos[j.node] for j in on] or [0],
+            other_pool_job_request=[_kubernetes_requirements(cfg, f, j.requests) for j in on] or [np.zeros(f.D)],
+            static_class_unschedulable=self.static_class_unschedulable, queue_limit_fraction=qf)
+        cs._keepalive = self.cluster_keep
+        self.cluster_state = cs
 
     def _queued_order(self, queued_order: Dict[str, List[str]]):
         """The caller's order of each queue's queued jobs: queues in index order, jobs by position."""
@@ -860,6 +979,107 @@ class RoundResult:
             if getattr(self.out, name) != getattr(other.out, name):
                 bad.append(f"{name}: {getattr(self.out, name)} vs {getattr(other.out, name)}")
         return bad
+
+
+def _field(inp, name: str, n: int) -> np.ndarray:
+    """Pointer field `name` of an ABI struct as a copy of its first n elements."""
+    ptr = getattr(inp, name)
+    return np.ctypeslib.as_array(ptr, (n,)).copy() if n and ptr else np.zeros(n, np.dtype(ptr._type_))
+
+
+class ClusterSnapshot:
+    """populateNodeDb (scheduling_algo.go:861-935) and NewSchedulingConstraints (constraints.go:94-111, 205-256)
+    restated on the ABI arrays: what armada_round_upload_cluster derives from (inp, cs).
+
+      input     the ArmadaRoundInput armada_round_upload takes for the same round: the kept nodes in the caller's
+                order with their id ranks among themselves, node flags, static classes and allocatable as derived,
+                job_node renumbered, the derived total and caps
+      kept      the caller's index of each node of `input`
+      snapshot  what armada_round_download_snapshot returns (the names of DeviceRound.download_snapshot)"""
+
+    def __init__(self, inp: abi.RoundInput, cs: abi.ClusterState):
+        N, D, J, K = inp.num_nodes, inp.num_resources, inp.num_jobs, cs.num_other_pool_jobs
+        Q, PC, S = inp.num_queues, inp.num_priority_classes, inp.num_static_classes
+        self.num_nodes = N
+        node_kube = np.array([not ((inp.floating_resource_mask >> d) & 1) for d in range(D)])
+        alloc_in = _field(inp, "node_allocatable", D * N).reshape(D, N)
+        flags_in = _field(inp, "node_flags", N)
+        sclass_in = _field(inp, "node_static_class", N)
+        req = _field(inp, "class_request", inp.num_classes * D).reshape(-1, D) * node_kube  # KubernetesResourceRequirements
+        jn = _field(inp, "job_node", J).astype(np.int64)
+        run = jn != abi.NONE
+        used = np.zeros((D, N), np.int64)
+        np.add.at(used.T, jn[run], req[_field(inp, "job_class", J).astype(np.int64)[run]])
+        pool_jobs = np.bincount(jn[run], minlength=N)
+        on = _field(cs, "other_pool_job_node", K).astype(np.int64)
+        oreq = _field(cs, "other_pool_job_request", K * D).reshape(K, D) * node_kube
+        other = np.zeros((D, N), np.int64)
+        np.add.at(other.T, on, oreq)
+        used += other
+        other_jobs = np.bincount(on, minlength=N)
+        unsched = (flags_in & abi.NODE_UNSCHEDULABLE) != 0
+        dropped = unsched & (pool_jobs == 0)  # no job of this pool: not inserted, not counted
+        exceeds = ~dropped & (pool_jobs + other_jobs > 0) & (used > alloc_in).any(axis=0)
+        scu = _field(cs, "static_class_unschedulable", S)
+        sclass = sclass_in.copy()
+        switch = exceeds & (scu[sclass_in] != abi.NONE)  # WithSchedulable(false) adds the taint, keeps the node type
+        sclass[switch] = scu[sclass_in[switch]]
+        marked = ~dropped & (other_jobs > 0)  # MarkResourceUnallocatable: allocatable - other pools, floored at zero
+        alloc = np.where(marked, np.maximum(alloc_in - other, 0), alloc_in)
+        state = (np.where(unsched, abi.NODE_UNSCHEDULABLE, 0) | np.where(exceeds, abi.NODE_UNSCHEDULABLE | abi.NODE_OVERALLOCATED, 0)
+                 | np.where(dropped, abi.NODE_DROPPED, 0)).astype(np.uint8)
+        kept = np.nonzero(~dropped)[0]
+        total = alloc[:, kept].sum(axis=1).astype(np.int64)
+        for d in range(D):
+            if (inp.floating_resource_mask >> d) & 1:
+                total[d] += inp.floating_limit[d]
+        max_sched = np.array([multiply_resource(int(total[d]), cs.max_fraction_to_schedule[d]) for d in range(D)], np.int64)
+        qf = _field(cs, "queue_limit_fraction", Q * PC * D).reshape(Q, PC, D) if cs.queue_limit_fraction else np.full((Q, PC, D), math.inf)
+        qlimit = np.array([[[multiply_resource(int(total[d]), float(qf[q, pc, d])) for d in range(D)] for pc in range(PC)] for q in range(Q)],
+                          np.int64).reshape(Q, PC, D)
+        self.kept = kept
+        self.snapshot = {"node_state": state, "node_allocatable": alloc, "node_static_class": sclass, "total_resources": total,
+                         "max_resources_to_schedule": max_sched, "queue_limit": qlimit}
+        # the equivalent explicit input
+        compact = np.full(N, abi.NONE, np.int64)
+        compact[kept] = np.arange(len(kept))
+        rank = _field(inp, "node_id_rank", N).astype(np.int64)
+        new_rank = np.empty(len(kept), np.uint32)
+        new_rank[np.argsort(rank[kept], kind="stable")] = np.arange(len(kept))
+        out = abi.RoundInput()
+        ctypes.memmove(ctypes.addressof(out), ctypes.addressof(inp), ctypes.sizeof(out))  # every field; node and job arrays replaced below
+        self._keep: List[np.ndarray] = []
+        out.num_nodes = len(kept)
+        nk = lambda a: a[:, kept] if a.ndim == 2 else a[kept]  # noqa: E731
+        abi.attach(out, self._keep, node_index=nk(_field(inp, "node_index", N)), node_id_rank=new_rank,
+                   node_type=nk(_field(inp, "node_type", N)), node_static_class=nk(sclass), node_flags=nk(state),
+                   node_total=nk(_field(inp, "node_total", D * N).reshape(D, N)), node_allocatable=nk(alloc),
+                   job_node=np.where(run, compact[np.where(run, jn, 0)], abi.NONE), queue_limit=qlimit)
+        out.has_round_limit = cs.has_round_limit
+        for d in range(D):
+            out.total_resources[d] = int(total[d])
+            out.max_resources_to_schedule[d] = int(max_sched[d])
+        out._keepalive = [inp, self._keep]
+        self.input = out
+
+    def in_caller_nodes(self, res: "RoundResult", inp: abi.RoundInput) -> "RoundResult":
+        """A RoundResult of `self.input`'s round in the caller's node numbering (the RoundResult of `inp`)."""
+        return result_in_caller_nodes(res, self.kept, inp)
+
+
+def result_in_caller_nodes(res: "RoundResult", kept, inp: abi.RoundInput) -> "RoundResult":
+    """A RoundResult over a pool's kept nodes (node k = the caller's node kept[k]) in the caller's node numbering, as
+    the RoundResult of `inp`, the round as reported: job_node mapped back, node_alloc columns of dropped nodes zero
+    (what armada_round_download leaves in a zeroed buffer)."""
+    kept = np.asarray(kept, np.int64)
+    out = RoundResult(inp, res.first_pass)
+    for name in RoundResult.ARRAYS + RoundResult.FIRST_PASS_ARRAYS:
+        getattr(out, name)[...] = getattr(res, name) if name != "node_alloc" else 0
+    out.node_alloc[:, :, kept] = res.node_alloc[:, :, : len(kept)]
+    out.job_node[...] = np.where(res.job_node == abi.NONE, abi.NONE, kept[np.where(res.job_node == abi.NONE, 0, res.job_node)])
+    for name in RoundResult.SCALARS:
+        setattr(out.out, name, getattr(res.out, name))
+    return out
 
 
 def node_preemptibility_stats(b: "RoundInputBuilder", res: "RoundResult") -> List[Tuple[str, bool, str]]:

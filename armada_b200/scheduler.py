@@ -36,6 +36,27 @@ class DeviceRound:
         _check(self.lib, self.lib.armada_round_upload(self.h, C.byref(inp)))
         self._input = inp
 
+    def upload_cluster(self, inp: abi.RoundInput, cs: abi.ClusterState) -> None:
+        """upload() with the pool's node set, total and caps derived on the device from the cluster as reported
+        (populateNodeDb + NewSchedulingConstraints; armada_round_upload_cluster)."""
+        _check(self.lib, self.lib.armada_round_upload_cluster(self.h, C.byref(inp), C.byref(cs)))
+        self._input = inp
+
+    def download_snapshot(self) -> dict:
+        """What the last upload_cluster derived, in the caller's node numbering: node_state [N] (abi.NODE_*),
+        node_allocatable [D][N], node_static_class [N], total_resources [D], max_resources_to_schedule [D],
+        queue_limit [Q][PC][D]."""
+        import numpy as np
+        inp = self._input
+        N, D, Q, PC = inp.num_nodes, inp.num_resources, inp.num_queues, inp.num_priority_classes
+        out = {"node_state": np.zeros(N, np.uint8), "node_allocatable": np.zeros((D, N), np.int64),
+               "node_static_class": np.zeros(N, np.uint32), "total_resources": np.zeros(D, np.int64),
+               "max_resources_to_schedule": np.zeros(D, np.int64), "queue_limit": np.zeros((Q, PC, D), np.int64)}
+        p = {k: v.ctypes.data_as(abi.u8p if v.dtype == np.uint8 else abi.u32p if v.dtype == np.uint32 else abi.i64p) for k, v in out.items()}
+        _check(self.lib, self.lib.armada_round_download_snapshot(self.h, p["node_state"], p["node_allocatable"], p["node_static_class"],
+                                                                 p["total_resources"], p["max_resources_to_schedule"], p["queue_limit"]))
+        return out
+
     def run(self, budget_ns: int = 0) -> abi.RoundStats:
         """`budget_ns` > 0: the cycle's maxSchedulingDuration (scheduling_algo.go:115-118); raises
         ArmadaError(E_DEADLINE) when it runs out — nothing of the round is committed."""

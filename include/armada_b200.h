@@ -135,6 +135,7 @@ typedef struct {
 /* node flags */
 #define ARMADA_NODE_UNSCHEDULABLE 1u /* Node.unschedulable (carries the unschedulable taint) */
 #define ARMADA_NODE_OVERALLOCATED 2u /* Node.overAllocated, scheduling_algo.go:911-916        */
+#define ARMADA_NODE_DROPPED 4u       /* armada_round_download_snapshot only: not in the NodeDb  */
 
 /* types.PriorityClass (internal/common/types/scheduling.go:56-76) reduced to what the
  * round reads. */
@@ -275,6 +276,30 @@ typedef struct {
   int64_t floating_limit[ARMADA_MAX_RESOURCES]; /* the pool's totals of the floating resources          */
 } ArmadaRoundInput;
 
+/* The pool as its executors report it, for armada_round_upload_cluster: what populateNodeDb
+ * (scheduling_algo.go:861-935) and NewSchedulingConstraints (constraints/constraints.go:94-111, 205-256)
+ * derive from it is derived on the device instead of being passed in ArmadaRoundInput. */
+typedef struct {
+  uint32_t abi_version;                       /* ARMADA_ABI_VERSION */
+  /* Jobs of OTHER pools running on this pool's nodes (populateNodeDb's otherPoolsJobs that are not terminal
+     and have a run).  They only take capacity: MarkResourceUnallocatable (node.go:285-294). */
+  uint32_t num_other_pool_jobs;               /* K */
+  const uint32_t* other_pool_job_node;        /* [K] node index of ArmadaRoundInput's nodes (jobs on nodes outside
+                                                 the pool are the caller's to skip)                              */
+  const int64_t* other_pool_job_request;      /* [K][D] KubernetesResourceRequirements, factory units           */
+  /* Static class of node static class s with the unschedulable taint added (what WithSchedulable(false) makes
+     of a node of class s, node.go:302-310), ARMADA_NONE where s carries it already.  static_match must have
+     columns for these classes; a node keeps its node type (the NodeDb keys by the type made at creation). */
+  const uint32_t* static_class_unschedulable; /* [S] */
+  /* calculatePerRoundLimits / calculatePerQueueLimits as fractions of the derived total; a missing fraction
+     is +Inf (multiplyResource saturates: no cap).  queue_has_limit of ArmadaRoundInput still says which
+     (queue, priority class) pairs have a cap. */
+  uint8_t has_round_limit;
+  uint8_t _pad[7];
+  double max_fraction_to_schedule[ARMADA_MAX_RESOURCES]; /* [D] */
+  const double* queue_limit_fraction;         /* [Q][PC][D], or NULL: no per-queue caps (every entry +Inf) */
+} ArmadaClusterState;
+
 /* All arrays are caller-allocated; any pointer may be NULL to skip that output. */
 typedef struct {
   uint8_t* job_state;            /* [J] ARMADA_JOB_*                                          */
@@ -357,6 +382,23 @@ int32_t armada_round_create(int32_t device, ArmadaRound** out);
 /* Validate + copy one round's inputs host→device (replaces NewNodeDb + populateNodeDb's
  * inputs + NewSchedulingContext/AddQueueSchedulingContext + InMemory/JobDb views). */
 int32_t armada_round_upload(ArmadaRound* r, const ArmadaRoundInput* in);
+/* armada_round_upload with the pool's node set derived on the device (populateNodeDb,
+ * scheduling_algo.go:861-935): per node the requests of this pool's running jobs and of cs's other-pool
+ * jobs; a node they Exceed becomes OVERALLOCATED and UNSCHEDULABLE (static class switched to
+ * static_class_unschedulable); the other pools' requests are taken off its allocatable, floored at zero;
+ * an UNSCHEDULABLE-as-reported node without a job of this pool is dropped.  The total is the kept nodes'
+ * allocatable plus floating_limit; max_resources_to_schedule and queue_limit follow from cs's fractions.
+ * In `in`: node_flags carries only ARMADA_NODE_UNSCHEDULABLE (cordoned, as reported), node_allocatable is
+ * Node.allocatableResources as reported; total_resources, max_resources_to_schedule, has_round_limit and
+ * queue_limit are ignored.  Run and download as after armada_round_upload, in the caller's node numbering:
+ * a dropped node is never probed, bound or counted, and download leaves its node_alloc entries untouched. */
+int32_t armada_round_upload_cluster(ArmadaRound* r, const ArmadaRoundInput* in, const ArmadaClusterState* cs);
+/* What the last armada_round_upload_cluster derived, in the caller's node numbering (any pointer may be NULL):
+ * node_state [N] ARMADA_NODE_* (ARMADA_NODE_DROPPED for a dropped node), node_allocatable [D][N] after
+ * MarkResourceUnallocatable, node_static_class [N], total_resources [D], max_resources_to_schedule [D],
+ * queue_limit [Q][PC][D].  ARMADA_E_STATE after any other upload. */
+int32_t armada_round_download_snapshot(ArmadaRound* r, uint8_t* node_state, int64_t* node_allocatable, uint32_t* node_static_class,
+                                       int64_t* total_resources, int64_t* max_resources_to_schedule, int64_t* queue_limit);
 /* Run PreemptingQueueScheduler.Schedule entirely on the device; inputs stay resident so
  * it can be called repeatedly (each call restarts from the uploaded snapshot). */
 int32_t armada_round_run(ArmadaRound* r, ArmadaRoundStats* stats);
@@ -428,8 +470,8 @@ int32_t armada_nodedb_destroy(ArmadaNodeDb* db);
 const char* armada_strerror(int32_t status);
 const char* armada_last_error(void);
 uint32_t armada_abi_version(void);
-/* sizeof() of the three boundary structs as compiled into the library (0 input, 1 output,
- * 2 stats); bindings check them against their own mirror of this header. */
+/* sizeof() of the boundary structs as compiled into the library (0 input, 1 output,
+ * 2 stats, 3 cluster state); bindings check them against their own mirror of this header. */
 uint32_t armada_abi_sizeof(uint32_t which);
 
 #ifdef __cplusplus

@@ -152,6 +152,20 @@ struct DevCfg {  // small POD, lives in global memory, hot parts copied to smem
   int64_t floating_limit[ARMADA_MAX_RESOURCES];
 };
 
+// one step of a gang's node transaction, undone by txn.Abort (Ctl::txn_abort in armada_pass.inc) in reverse order
+enum UndoKind : uint32_t {
+  UNDO_BIND = 1,        // bindJobToNodeInPlace of a job onto `node`
+  UNDO_REBIND_EVICTED,  // the same for an evicted jctx re-bound to its own node
+  UNDO_UNBIND_VICTIM,   // unbindJobFromNodeInPlace of a fair-preemption victim evicted from `node`
+  UNDO_DROP_EVICTED,    // deleteEvictedJobSchedulingContextIfExistsWithTxn (node unused)
+};
+struct UndoRec {
+  uint32_t kind, job, node;
+  uint32_t arg;  // bind and re-bind: the priority bound at (int32_t); unbind and drop: the jctx's evicted index
+  uint32_t cls;
+};
+static_assert(sizeof(UndoRec) == 20, "five words per undo record");
+
 struct DevPtrs {
   // ---- immutable snapshot (uploaded once per round input) ----
   const int64_t* node_total;       // [D][N]
@@ -254,7 +268,7 @@ struct DevPtrs {
   const uint8_t* gang_simple;      // [G] every member queued, complete, one class, contiguous in its queue (batchable)
   uint32_t* excl;                  // [J][ARMADA_EXCLUDED_KINDS] NumExcludedNodesByReason by kind of the failed single jobs (collect_excl)
   const uint32_t* row_type_excl;   // [rows] nodes of the node types the row does not match (NodeTypesMatchingJob)
-  uint32_t* undo_log;              // [5 * J] txn undo records
+  UndoRec* undo_log;               // [3 * J + 16] txn undo records
   // fair preemption scratch
   uint32_t* fp_head;               // [N] most recent visited evicted index on the node
   uint32_t* fp_next;               // [J] chain by evicted index

@@ -14,8 +14,11 @@ from armada_b200.scheduler import DeviceRound
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 EMU_DIR = os.path.join(ROOT, "tools", "simt_emu")
-EMU_LIB = os.path.join(EMU_DIR, "libarmada_b200_emu.so")
 CSRC = os.path.join(ROOT, "armada_b200", "csrc")
+# ARMADA_EMU_COVERAGE=1 (tools/emu_coverage.py): a --coverage build under its own name, so that the plain library
+# and its build command stay as they are
+COVERAGE = os.environ.get("ARMADA_EMU_COVERAGE") == "1"
+EMU_LIB = os.path.join(EMU_DIR, "libarmada_b200_emu_cov.so" if COVERAGE else "libarmada_b200_emu.so")
 _lib = None
 
 
@@ -32,11 +35,14 @@ def build(force: bool = False) -> None:
         fcntl.flock(lock, fcntl.LOCK_EX)
         if force or stale():
             tmp = f"{EMU_LIB}.{os.getpid()}.tmp"
+            # coverage: the counters are named after the output file, so it is built under its final name
+            out = EMU_LIB if COVERAGE else tmp
             subprocess.run(
                 ["g++", "-O1", "-g", "-std=c++17", "-fPIC", "-shared", "-ffp-contract=off", "-DARMADA_EMU", "-x", "c++",
                  os.path.join(CSRC, "armada_round.cu"), "-I", os.path.join(ROOT, "include"), "-I", CSRC, "-I", EMU_DIR,
-                 "-o", tmp, "-lpthread"], check=True)
-            os.replace(tmp, EMU_LIB)
+                 "-o", out, "-lpthread"] + (["--coverage"] if COVERAGE else []), check=True)
+            if not COVERAGE:
+                os.replace(tmp, EMU_LIB)
 
 
 def load() -> C.CDLL:
